@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the HumanRF per-ray hot path on B200 (see DESIGN.md "Measurement").
+"""bench.py -- headline benchmark of the HumanRF per-ray hot path on H100 (see DESIGN.md "Measurement").
 
-BASELINE.json's metric is "train rays/sec & render Mpix/s at 1/2/4/8 B200".  A step = one pass of the hot path over one
+BASELINE.json's metric is "train rays/sec & render Mpix/s" at 1/2/4/8 GPUs.  A step = one pass of the hot path over one
 synthetic batch (SURVEY 8d / BASELINE.md section 2): 4096 rays x 512 samples = 2,097,152 candidate samples per GPU,
 segment_sizes=(50,) (log2T=18), 8 distinct frames of 15..64:
     --mode train (default, configs[2]): jitter + prune pass (early-stop density over all candidates, keeps the composed
@@ -15,13 +15,17 @@ segment_sizes=(50,) (log2T=18), 8 distinct frames of 15..64:
 `value` is timed with CUDA events per step (inputs resident in HBM, L2 flushed between steps); `e2e` goes through the
 public API (FusedTrainer.step / volume_rendering.render) with pinned HOST buffers, H2D and D2H inside the timed region.
 The default (train) line at N=1 also carries `render` and `image` (each measured in its own process right after).
+`--steps` is the number of timed steps of every loop (the event-timed window, the e2e loop and the companions).
+`--dump-outputs DIR` (train / render) writes what the last timed step computed as DIR/<name>.npy (float32 / float64, a
+fixed seeded sample of the large tensors, < 64 MB in all); the inputs are seeded, so two builds can be compared output by
+output.
 `--impl reference` times the CPU oracle port of the same path (the reference's tcnn/nerfacc path is CUDA-only and not
 installable here) on the box's host cores.
 """
 from __future__ import annotations
 
 import argparse
-import csv
+import atexit
 import json
 import os
 import subprocess
@@ -50,44 +54,7 @@ def load_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         return float(json.loads(p.read_text())["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
-
-
-def committed_ncu(kernel_substr):
-    """Per-launch figures of a kernel from the newest committed `ncu --set full` export under profiles/ that contains it
-    (a measurement, not a constant in this file): DRAM bytes, L1TEX / L2 throughput %, issue-slot %."""
-    unit_scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    for f in sorted((ROOT / "profiles").glob("r2*_ncu_full_*_raw.csv"), key=lambda p: p.name, reverse=True):
-        try:
-            rows = list(csv.reader(open(f)))
-        except OSError:
-            continue
-        if len(rows) < 3:
-            continue
-        h, units = rows[0], rows[1]
-        for r in rows[2:]:
-            d = dict(zip(h, r))
-            if kernel_substr not in d.get("Kernel Name", ""):
-                continue
-            u = dict(zip(h, units))
-
-            def num(k, scale=False):
-                try:
-                    v = float(d[k].replace(",", ""))
-                except (KeyError, ValueError):
-                    return None
-                return v * unit_scale.get(u.get(k, ""), 1.0) if scale else v
-
-            rd, wr = num("dram__bytes_read.sum", True), num("dram__bytes_write.sum", True)
-            return {"traffic": None if rd is None or wr is None else rd + wr, "source": f"profiles/{f.name}",
-                    "kernel_name": d["Kernel Name"],
-                    "l1tex_pct": num("l1tex__throughput.avg.pct_of_peak_sustained_active"),
-                    "l2_pct": num("lts__throughput.avg.pct_of_peak_sustained_elapsed"),
-                    "dram_pct": num("gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed"),
-                    "issue_slots_pct": num("smsp__issue_active.avg.pct_of_peak_sustained_active"),
-                    "tensor_pipe_pct": num("sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"),
-                    "ncu_duration_ms": num("gpu__time_duration.sum")}
-    return None
+    return 3350.0, "fallback: H100 SXM data sheet HBM3 bandwidth"
 
 
 class ClockSampler:
@@ -101,6 +68,8 @@ class ClockSampler:
                                           "-lms", "20"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
         except Exception:  # noqa: BLE001
             self.proc = None
+        if self.proc is not None:   # never leave the sampler running, whatever ends this process
+            atexit.register(self.proc.kill)
 
     def stop(self):
         if self.proc is None:
@@ -127,6 +96,26 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def _sample(x, n, seed):
+    """A fixed, seeded sample of n entries of x (all of x when it is smaller), as a float32 / float64 numpy array."""
+    x = x.detach().reshape(-1)
+    if x.numel() > n:
+        g = torch.Generator(device=x.device).manual_seed(seed)
+        x = x[torch.randint(0, x.numel(), (n,), device=x.device, generator=g)]
+    return x.cpu().numpy().astype("float64" if x.dtype == torch.float64 else "float32")
+
+
+def dump_outputs(out_dir, arrays):
+    import numpy as np
+
+    out_dir = Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 * 2 ** 20, total
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def build_workload(device, seed):
@@ -161,7 +150,7 @@ def companion_line(mode, steps):
         keep["e2e"] = (full.get("e2e") or {}).get("value")
         keep["workload"] = (full.get("config") or {}).get("workload")
         if full.get("roofline"):
-            keep["roofline"] = {k: full["roofline"].get(k) for k in ("kernel", "frac", "achieved", "kernel_ms", "traffic")}
+            keep["roofline"] = {k: full["roofline"].get(k) for k in ("kernel", "frac", "achieved", "kernel_ms")}
         return keep
     except Exception as e:  # noqa: BLE001 -- the headline line must still be printed
         return {"error": f"{type(e).__name__}: {e}"[:300]}
@@ -311,7 +300,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-companions", action="store_true",
                     help="do not append the render / full-image numbers to the default train line")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (train and render modes)")
     args = ap.parse_args()
+    if args.dump_outputs and args.mode not in ("train", "render"):
+        ap.error("--dump-outputs is supported in the train and render modes")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -356,13 +349,15 @@ def main():
         trainer.profile = True
     g = {k: v.to(dev).contiguous() for k, v in b.items() if k in ("o", "d", "frames", "t", "ri", "rgba")}
     n = g["t"].shape[0]
-    bg = torch.rand(RAYS, 3, device=dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    bg = torch.rand(RAYS, 3, device=dev, generator=torch.Generator(device=dev).manual_seed(7))
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     off_all = ray_offsets(g["ri"], RAYS)
     launches = {"n": 0}
+    rendered = {}
 
     def step_render(ev=None):
-        render_fused(model, g["o"], g["d"], g["frames"], g["t"], g["ri"], RAYS, bg, ray_offsets_dev=off_all)
+        rendered["color"], rendered["weights_sum"] = render_fused(model, g["o"], g["d"], g["frames"], g["t"], g["ri"], RAYS, bg,
+                                                                  ray_offsets_dev=off_all)
         if ev is not None:
             ev.record()
         launches["n"] += 2
@@ -397,6 +392,15 @@ def main():
         ev[i][2].record()
     barrier()
     t_wall = time.perf_counter() - t_wall
+    if args.dump_outputs and rank == 0:
+        if args.mode == "render":
+            dump_outputs(args.dump_outputs, {k: _sample(v, 1 << 20, 0) for k, v in rendered.items()})
+        else:   # the loss, the Adam moments (the gradients' trace) and the updated parameters after the last timed step
+            arrays = {"loss": _sample(trainer.last["loss"], 1, 0), "samples_after_prune": _sample(torch.as_tensor(trainer.last["samples"], dtype=torch.float64), 1, 0),
+                      "adam_exp_avg": _sample(trainer.exp_avg, 2 << 20, 1), "adam_exp_avg_sq": _sample(trainer.exp_avg_sq, 2 << 20, 2)}
+            for i, p in enumerate(model.hot_parameters()):
+                arrays[f"param{i}"] = _sample(p, 1 << 20, 3 + i)
+            dump_outputs(args.dump_outputs, arrays)
     step_ms = sum(e[0].elapsed_time(e[2]) for e in ev)
     kern_ms = sum(e[0].elapsed_time(e[1]) for e in ev) / args.steps
     tt = torch.tensor([step_ms], device=dev, dtype=torch.float64)
@@ -423,9 +427,7 @@ def main():
     # ---- e2e through the public API with pinned host buffers -------------------------------------
     host = {k: b[k].contiguous().pin_memory() for k in ("o", "d", "frames", "t", "ri", "rgba")}
     # The ray index of a sample travels as int32 (FusedTrainer.step / volume_rendering.render widen it on the device): 8
-    # instead of 17 MB per step.  With int64 the 25 MB upload needs 10.8 GB/s to hide behind a 2.35 ms train step (24 GB/s
-    # behind a 1.03 ms render step), which not every host of this pool sustains from pinned memory: the train e2e moved
-    # 1.54-1.72 M rays/s from box to box (profiles/r2k-r2n).
+    # instead of 17 MB per step, so the upload hides behind the step on hosts with less pinned-memory bandwidth.
     host["ri"] = b["ri"].to(torch.int32).contiguous().pin_memory()
     host_color = torch.empty(RAYS, 3).pin_memory()
     h2d = sum(host[k].numel() * host[k].element_size() for k in ("o", "d", "frames", "t", "ri"))
@@ -433,8 +435,8 @@ def main():
 
     from humanrf_b200.dataset.input_batch import InputBatch
 
-    # Render: three steps in flight on three streams (one pinned->device stream sustains ~16 GB/s on this host,
-    # scripts/e2e_probe.py), so step i+1's H2D copy and step i-1's D2H read overlap step i's kernels (copy engines beside
+    # Render: three steps in flight on three streams (scripts/e2e_probe.py measures one pinned->device stream), so step
+    # i+1's H2D copy and step i-1's D2H read overlap step i's kernels (copy engines beside
     # the SMs) -- how a renderer walks the tiles of an image.  Train: steps are sequentially dependent (Adam), so the next
     # batch's H2D copy is prefetched on a copy stream and the loss of step i is read back (pinned, asynchronously) while
     # step i+1 runs.  Every step's copies are issued, and complete, inside the timed region.
@@ -466,8 +468,8 @@ def main():
     # Train: two resident device batches; batch i+1 is copied from pinned host memory on the copy stream while step i runs
     # (the copy waits until the step that last read that buffer has finished, the step waits for its copy).
     dev_batches = [{k: torch.empty_like(host[k], device=dev) for k in keys} for _ in range(2)]
-    # (the copy is split over two streams / copy engines: one pinned->device stream alone sustains 10-16 GB/s on this host,
-    #  and 25 MB per step then take longer than the 2.3 ms step they hide behind)
+    # (the copy is split over two streams / copy engines: one pinned->device stream alone may take longer than the step
+    #  it hides behind)
     lanes = (("ri",), tuple(k for k in keys if k != "ri"))
     copied = [[torch.cuda.Event() for _ in lanes] for _ in range(2)]
     consumed = [torch.cuda.Event() for _ in range(2)]
@@ -502,7 +504,7 @@ def main():
     e2e_loop(5)
     barrier()
     t0 = time.perf_counter()
-    k_e2e = max(50, args.steps)
+    k_e2e = args.steps
     e2e_loop(k_e2e)
     barrier()
     e2e_s = time.perf_counter() - t0
@@ -522,21 +524,17 @@ def main():
         if args.mode == "render":
             alg_per_sample, roof_kernel = ALG_BYTES_FWD, "field_forward_kernel<composite epilogue> (+ composite_fixup_kernel)"
             achieved = alg_per_sample * n / (kern_ms * 1e-3) / 1e9
-            prof = committed_ncu("field_forward_kernel")
-            note = ("SURVEY 8d convention: table gathers served by L2 count as algorithmic bytes; the physical limiter is the "
-                    "L1/TEX gather pipe, see l1tex_pct / issue_slots_pct")
+            note = "SURVEY 8d convention: table gathers served by L2 count as algorithmic bytes"
         else:
             # dominant kernel of the train step: the table-gradient scatter over the pruned samples
-            gen = os.environ.get("HRF_SCATTER", "3")      # the library's default generation (csrc/field_bwd.cu HRF_SCATTER_DEFAULT)
-            gen = gen if gen in ("2", "3", "4", "5") else "3"
+            gen = os.environ.get("HRF_SCATTER", "5")      # the library's default generation (csrc/field_bwd.cu HRF_SCATTER_DEFAULT)
+            gen = gen if gen in ("2", "3", "4", "5") else "5"
             alg_per_sample, roof_kernel = ALG_BYTES_SCATTER, f"grid_scatter_v{gen}_kernel"
             kern_ms = phases.get("scatter", 0.0)
             achieved = alg_per_sample * kept_mean / max(kern_ms * 1e-3, 1e-9) / 1e9
-            prof = committed_ncu(roof_kernel)
             note = ("SURVEY 8d backward convention: 2 x 2048 B table-gradient RMW + 2 x 1024 B vector-gradient RMW per surviving "
                     "sample; the RMWs are L2 atomics (red.global.add.v2.f32) that run-length and warp-level combining keep off "
-                    "DRAM, so the convention's bytes are not physical traffic (see traffic); physical limiters: L1TEX RED "
-                    "wavefronts, L2 RED requests, issue slots (l1tex_pct / l2_pct / issue_slots_pct)")
+                    "DRAM, so the convention's bytes are not physical traffic")
         line = {
             "metric": METRIC[args.mode], "value": value, "unit": "rays/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": total_ms / args.steps, "higher_is_better": True,
@@ -552,11 +550,8 @@ def main():
             "gpu_launches": gpu_launches,
             "clocks": clk,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": prof["traffic"] if prof else None, "traffic_unit": "bytes/launch",
-                         "traffic_source": prof["source"] if prof else None,
                          "peak_source": which, "kernel": roof_kernel, "kernel_ms": kern_ms,
-                         "algorithmic_bytes_per_sample": alg_per_sample, "note": note,
-                         **({k: prof[k] for k in ("l1tex_pct", "l2_pct", "dram_pct", "issue_slots_pct", "tensor_pipe_pct")} if prof else {})},
+                         "algorithmic_bytes_per_sample": alg_per_sample, "note": note},
             "wall_s_timed_loop": t_wall,
         }
         if args.mode == "train":
@@ -582,7 +577,7 @@ def main():
             # BASELINE.json's metric is a pair ("train rays/sec & render Mpix/s"): the other two workloads run right after
             # (each in its own process, own timed region, same rules) and are attached so one run reports all three.
             line["render"] = companion_line("render", args.steps)
-            line["image"] = companion_line("image", 5)
+            line["image"] = companion_line("image", args.steps)
             line["config"]["render_rays_per_s"] = line["render"].get("value")
             line["config"]["render_mpix_per_s"] = line["image"].get("value")
         print(json.dumps(line))

@@ -1,4 +1,4 @@
-"""humanrf_b200 -- B200-native (sm_100a) implementation of HumanRF's per-ray hot path.
+"""humanrf_b200 -- H100-native (sm_90a) implementation of HumanRF's per-ray hot path.
 
 Host-side mirror of the reference's interfaces for that path (same names, argument meaning and
 error behaviour) on top of the C ABI in include/humanrf_b200.h:

@@ -1,4 +1,4 @@
-"""Builds libhumanrf_b200.so (sm_100a) in-tree with nvcc.  No torch involvement: the library is
+"""Builds libhumanrf_b200.so (sm_90a) in-tree with nvcc.  No torch involvement: the library is
 a plain C-ABI shared object (include/humanrf_b200.h).  Every .cu is compiled to its own object file (in parallel,
 re-done only when that file, a header or the flags change), then linked."""
 from __future__ import annotations
@@ -16,7 +16,7 @@ LIB = PKG / "libhumanrf_b200.so"
 STAMP = PKG / ".libhumanrf_b200.stamp"
 OBJ = PKG / "build"
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -73,7 +73,7 @@ def build_library(force: bool = False, verbose: bool = False) -> Path:
         sys.stderr.write(log)
         raise RuntimeError("nvcc failed building libhumanrf_b200.so (see humanrf_b200/build.log)")
     tmp = LIB.with_suffix(".so.tmp")      # linked beside, then renamed: a reader never sees a half-written library
-    res = subprocess.run([nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC", "-o", str(tmp),
+    res = subprocess.run([nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC", "-o", str(tmp),
                           *[str(OBJ / (s.stem + ".o")) for s in srcs]], capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)

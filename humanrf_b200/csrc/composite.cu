@@ -1,4 +1,4 @@
-// Per-ray transmittance scans, visibility pruning and alpha compositing for sm_100a.
+// Per-ray transmittance scans, visibility pruning and alpha compositing for sm_90a.
 // Replaces the nerfacc 0.3.1 calls of humanrf/volume_rendering.py:75-84,123-145
 // (render_visibility, render_weight_from_density, accumulate_along_rays) and their backward.
 // One warp owns one ray; transmittance is a warp-shuffle prefix scan with a running carry,

@@ -1,17 +1,17 @@
-// Fused backward of the HumanRF radiance field for sm_100a (autograd of humanrf.py:158-208).
-// Per 128-sample tile (thread r = sample r = operand row r = TMEM lane r):
+// Fused backward of the HumanRF radiance field for sm_90a (autograd of humanrf.py:158-208).
+// Per 128-sample tile (thread r = sample r = operand row r; the CTA is one warpgroup):
 //   1. forward recompute of both MLPs from the saved composed features (or a re-encode),
-//      keeping every activation tile in shared memory (bf16, UMMA K-major core-matrix layout);
-//   2. MLP backward on the tensor cores.  The SAME shared-memory tiles serve three roles by
+//      keeping every activation tile in shared memory (bf16, K-major core-matrix layout);
+//   2. MLP backward on the tensor cores (wgmma).  The SAME shared-memory tiles serve three roles by
 //      switching descriptors only:  K-major A operand of the forward / dgrad GEMMs, and
 //      MN-major A / B operands of the wgrad GEMMs (contraction over the 128 samples).  The
 //      packed forward weight blob is re-used as the MN-major B operand of the dgrad GEMMs.
-//      Weight-gradient accumulators live in TMEM for the whole persistent CTA (M=64 tiles)
-//      and are flushed once with fp32 atomics;
+//      Weight-gradient accumulators (M=64 each, 88 registers a thread) live in registers for the whole
+//      persistent CTA and are flushed once with fp32 atomics;
 //   3. d(composed features) goes to a level-major [16][N] workspace; a second, high-occupancy kernel
 //      (grid_scatter_kernel: thread = (sample, level)) re-gathers the 4x8 corners (needed for the vector
 //      gradients) and issues red.global.add.v2.f32 into the fp32 table gradients, with warp-combined adds
-//      for the time axis.  (One fused kernel was latency-bound at 12.5 % occupancy: profiles/r1_ncu_full_bwd.)
+//      for the time axis.  (One fused kernel was latency-bound at its low occupancy.)
 #include <cstddef>
 #include <cstdlib>
 
@@ -25,21 +25,11 @@ struct __align__(1024) BwdSmem {
   unsigned char cin[kTile * 48 * 2];   // colour-net input              (A32 / A48)
   unsigned char hs[kTile * 64 * 2];    // sigma hidden, then d(hidden)  (A64)
   unsigned char h1[kTile * 64 * 2];    // colour hidden 1, then its gradient, then dFeat staging
-  unsigned char h2[kTile * 64 * 2];    // colour hidden 2, then its gradient
+  unsigned char h2[kTile * 64 * 2];    // colour hidden 2, then its gradient, then d(colour input) staging
   unsigned char g3[kTile * 16 * 2];    // d(colour pre-activation)  [128,16]
-  unsigned char gs[kTile * 16 * 2];    // d(sigma-net output)       [128,16]
-  uint64_t bar_w, bar_mma;
-  uint32_t tmem_base;
+  unsigned char gs[kTile * 16 * 2];    // colour-net output staging, then d(sigma-net output) [128,16]
+  uint64_t bar_w;
 };
-
-// TMEM column map (256 columns allocated): work area + persistent weight-gradient accumulators
-constexpr uint32_t kColWork = 0;     // 64 cols: layer outputs / dgrad results
-constexpr uint32_t kColW1s = 64;     // dW1s   [64 out, 32 in]
-constexpr uint32_t kColW2s = 96;     // dW2s^T [64 in, 16 out]
-constexpr uint32_t kColW1c = 112;    // dW1c   [64 out, 32|48 in]
-constexpr uint32_t kColW2c = 160;    // dW2c   [64 out, 64 in]
-constexpr uint32_t kColW3c = 224;    // dW3c^T [64 in, 16 out]
-constexpr uint32_t kTmemCols = 256;
 
 struct BwdArgs {
   hrf_field f;
@@ -58,68 +48,42 @@ struct BwdArgs {
 };
 
 // D[128,Nin] = G[128,Kout] * W[Kout,Nin]  : A = gradient tile (K-major), B = forward blob read MN-major
-__device__ __forceinline__ void issue_dgrad(uint32_t tmem_d, uint32_t g_addr, uint32_t w_addr, int Nin, int Kout) {
-  const uint32_t idesc = make_idesc_bf16(kTile, Nin, 0, 1);
-  const uint32_t b_sbo = (uint32_t)(Kout >> 3) * 128u;
+template <int Nin, int Kout>
+__device__ __forceinline__ void issue_dgrad(float* d, uint32_t g_addr, uint32_t w_addr) {
+  constexpr uint32_t b_sbo = (uint32_t)(Kout >> 3) * 128u;
+#pragma unroll
   for (int k = 0; k < Kout / 16; ++k) {
-    const uint64_t ad = make_smem_desc(g_addr + (uint32_t)k * 2u * kAChunk, kAChunk, 128u);
     const uint64_t bd = make_smem_desc(w_addr + (uint32_t)k * 256u, 128u, b_sbo);
-    umma_bf16(tmem_d, ad, bd, idesc, k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      wgmma_bf16<Nin, 0, 1>(d + h * (Nin / 2), make_smem_desc(g_addr + h * kAHalf + (uint32_t)k * 2u * kAChunk, kAChunk, 128u),
+                            bd, k > 0 ? 1u : 0u);
   }
 }
-// D[64,N] (+)= X^T[64,128] * Y[128,N] : both tiles read MN-major, contraction over the 128 samples
-__device__ __forceinline__ void issue_wgrad(uint32_t tmem_d, uint32_t x_addr, uint32_t y_addr, int N, bool acc) {
-  const uint32_t idesc = make_idesc_bf16(64, N, 1, 1);
+// D[64,N] += X^T[64,128] * Y[128,N] : both tiles read MN-major, contraction over the 128 samples
+template <int N>
+__device__ __forceinline__ void issue_wgrad(float* d, uint32_t x_addr, uint32_t y_addr) {
+#pragma unroll
   for (int k = 0; k < kTile / 16; ++k) {
     const uint64_t ad = make_smem_desc(x_addr + (uint32_t)k * 256u, 128u, kAChunk);
     const uint64_t bd = make_smem_desc(y_addr + (uint32_t)k * 256u, 128u, kAChunk);
-    umma_bf16(tmem_d, ad, bd, idesc, (acc || k > 0) ? 1u : 0u);
+    wgmma_bf16<N, 1, 1>(d, ad, bd, 1u);
   }
 }
 
-template <class F>
-__device__ __forceinline__ void mma_round(BwdSmem& sm, uint32_t& phase, F&& issue) {
-  tc_fence_before();
-  fence_proxy_async_smem();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    tc_fence_after();
-    issue();
-    umma_commit(&sm.bar_mma);
-  }
-  mbar_wait(&sm.bar_mma, phase);
-  phase ^= 1u;
-  tc_fence_after();
-}
-
-// store relu(v) as a K=64 bf16 tile row
-__device__ __forceinline__ void store_relu64(unsigned char* buf, uint32_t roff, const float* v) {
+// in place: the tile holds relu(h) (bf16, K = 64); replace it by D * (h > 0) (bf16), D[128,64] in fragments
+__device__ __forceinline__ void frag_relu_backward64(unsigned char* buf, const float* d) {
 #pragma unroll
-  for (int kg = 0; kg < 8; ++kg) {
-    uint4 q;
-    q.x = pack_bf16x2(fmaxf(v[kg * 8 + 0], 0.f), fmaxf(v[kg * 8 + 1], 0.f));
-    q.y = pack_bf16x2(fmaxf(v[kg * 8 + 2], 0.f), fmaxf(v[kg * 8 + 3], 0.f));
-    q.z = pack_bf16x2(fmaxf(v[kg * 8 + 4], 0.f), fmaxf(v[kg * 8 + 5], 0.f));
-    q.w = pack_bf16x2(fmaxf(v[kg * 8 + 6], 0.f), fmaxf(v[kg * 8 + 7], 0.f));
-    *reinterpret_cast<uint4*>(buf + kg * kAChunk + roff) = q;
-  }
-}
-// in place: tile row holds relu(h) (bf16); replace by g * (h > 0) (bf16)
-__device__ __forceinline__ void relu_backward_inplace64(unsigned char* buf, uint32_t roff, const float* g) {
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-  for (int kg = 0; kg < 8; ++kg) {
-    uint4* p = reinterpret_cast<uint4*>(buf + kg * kAChunk + roff);
-    const uint4 a = *p;
-    const uint32_t av[4] = {a.x, a.y, a.z, a.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float lo = (av[j] & 0x7fffu) != 0u && !(av[j] & 0x8000u) ? g[kg * 8 + 2 * j] : 0.f;
-      const float hi = (av[j] & 0x7fff0000u) != 0u && !(av[j] & 0x80000000u) ? g[kg * 8 + 2 * j + 1] : 0.f;
-      o[j] = pack_bf16x2(lo, hi);
+    for (int q = 0; q < 32; q += 2) {
+      const int r = frag_row(h, q), c = frag_col(q);
+      uint32_t* p = reinterpret_cast<uint32_t*>(buf + (c >> 3) * kAChunk + a_row_off(r) + (c & 7) * 2);
+      const uint32_t a = *p;
+      const float lo = (a & 0x7fffu) != 0u && !(a & 0x8000u) ? d[h * 32 + q] : 0.f;
+      const float hi = (a & 0x7fff0000u) != 0u && !(a & 0x80000000u) ? d[h * 32 + q + 1] : 0.f;
+      *p = pack_bf16x2(lo, hi);
     }
-    *p = make_uint4(o[0], o[1], o[2], o[3]);
-  }
 }
 
 __device__ __forceinline__ float warp_sum_f(float v) {
@@ -131,8 +95,24 @@ __device__ __forceinline__ void red_add2(float* addr, float a, float b) {
   // no return value wanted: the vector RED, not the ATOM the float2 atomicAdd intrinsic compiles to
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {   // addr 16-byte aligned
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+
+// Flush of an M = 64 weight-gradient fragment D (kRegs registers): dst[m * ld + c] += D[m][c] for c < n, the two
+// adjacent columns a thread holds as one 8-byte RED when dst is 8-byte aligned.
+template <int kRegs>
+__device__ __forceinline__ void flush_rows(float* dst, int ld, const float* acc, int n, bool v2ok) {
+#pragma unroll
+  for (int q = 0; q < kRegs; q += 2) {
+    const int m = frag_row(0, q), c = frag_col(q);
+    if (c < n) {
+      if (v2ok) red_add2(dst + m * ld + c, acc[q], acc[q + 1]);
+      else atomicAdd(dst + m * ld + c, acc[q]), atomicAdd(dst + m * ld + c + 1, acc[q + 1]);
+    }
+  }
+}
+// Transposed flush of an M = 64, N = 16 fragment: dst[c * 64 + m] += D[m][c].
+__device__ __forceinline__ void flush_cols(float* dst, const float* acc) {
+#pragma unroll
+  for (int q = 0; q < 8; ++q) atomicAdd(dst + frag_col(q) * 64 + frag_row(0, q), acc[q]);
 }
 
 // Moving to the neighbouring cell along one axis (bit kBit of the corner number) keeps the face the two cells share:
@@ -165,7 +145,7 @@ __device__ __forceinline__ void shift_corners(int d, float* gtab, uint32_t (&idx
 // the L2 atomics and the gathers by the run length (about 80 samples at level 0, 1.2 at level 15) with no
 // shuffles.  Each grid pairs with exactly one vector axis (xyz<->t, xyt<->z, yzt<->x, xzt<->y), so the
 // (level, grid) threads are independent.
-constexpr int kChunkDefault = 16;  // samples per thread (HRF_SCATTER_CHUNK overrides; measured 8 -> 4.02, 16 -> 3.73, 32 -> 3.79 ms backward)
+constexpr int kChunkDefault = 16;  // samples per thread (HRF_SCATTER_CHUNK overrides)
 
 struct ScatterArgs {
   hrf_field f;
@@ -304,8 +284,7 @@ __global__ void __launch_bounds__(256, 3) grid_scatter_kernel(const __grid_const
 
 // ---- staged variant (the default) --------------------------------------------------------------------------------
 // grid_scatter_kernel reads its per-sample inputs with a stride of `chunk` samples between lanes, so every 32-byte
-// sector is fetched for 16 / 8 / 4 / 1 useful bytes and the ~400 KB of streams per SM thrash L1 (ncu, 16 samples
-// per thread: L1 hit 20 %, L1/TEX throughput 79 %, L2 RED sectors only 20 % of peak -- profiles/r1_ncu_scatter_*).
+// sector is fetched for 16 / 8 / 4 / 1 useful bytes and the ~400 KB of streams per SM thrash L1.
 // Here a CTA of 128 threads owns 1024 consecutive samples: positions and segment ids are staged in shared memory
 // once with coalesced loads and re-used for kStLevels levels; per level the d(feature) row and the saved grid
 // features are staged the same way.  Each thread then walks its 8 consecutive samples out of shared memory
@@ -508,27 +487,27 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
 
   if (tid == 0) {
     mbar_init(&sm.bar_w, 1);
-    mbar_init(&sm.bar_mma, 1);
     fence_mbar_init();
   }
-  if (tid < 32) {
-    tmem_alloc(&sm.tmem_base, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   if (tid == 0) {
     mbar_arrive_expect_tx(&sm.bar_w, w_blob_bytes(f.color_in_width));
     tma_load_1d(sm.w, f.mlp_blob, w_blob_bytes(f.color_in_width), &sm.bar_w);
   }
-  const uint32_t tm = sm.tmem_base;
-  const uint32_t trow = tm + ((uint32_t)(tid & ~31) << 16);  // this warp's TMEM lanes
   const uint32_t wbase = smem_u32(sm.w);
   const uint32_t a_feat = smem_u32(sm.feat), a_cin = smem_u32(sm.cin), a_hs = smem_u32(sm.hs),
                  a_h1 = smem_u32(sm.h1), a_h2 = smem_u32(sm.h2), a_g3 = smem_u32(sm.g3), a_gs = smem_u32(sm.gs);
   bool weights_ready = false, have_acc = false;
-  uint32_t phase = 0;
+  // weight-gradient accumulators, M = 64 wgmma fragments (see wgmma_bf16), summed over every tile of the CTA
+  float gw1s[16], gw2s[8], gw1c[24], gw2c[32], gw3c[8];   // dW1s [64 out,32 in], dW2s^T [64 in,16 out],
+#pragma unroll                                             // dW1c [64 out,K1 in], dW2c [64,64], dW3c^T [64 in,16 out]
+  for (int q = 0; q < 32; ++q) {
+    if (q < 16) gw1s[q] = 0.f;
+    if (q < 8) gw2s[q] = 0.f, gw3c[q] = 0.f;
+    if (q < 24) gw1c[q] = 0.f;
+    gw2c[q] = 0.f;
+  }
+  const int K1 = f.color_in_width;
 
   const int64_t n = live_samples(args.s);
   const int64_t ns = args.s.num_samples;   // row length of the level-major workspace
@@ -563,24 +542,40 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
       mbar_wait(&sm.bar_w, 0);
       weights_ready = true;
     }
-    float v[64], o[16];
+    float d[64], o[16];
     // ---------------- forward recompute ----------------
-    mma_round(sm, phase, [&] { issue_layer(tm + kColWork, a_feat, wbase + kWSig1, 64, 32); });
-    tmem_ld64(trow + kColWork, v);
-    store_relu64(sm.hs, roff, v);
-    mma_round(sm, phase, [&] { issue_layer(tm + kColWork, a_hs, wbase + kWSig2, 16, 64); });
-    tmem_ld16(trow + kColWork, o);
+    mma_begin();
+    mma_layer<64, 32>(d, a_feat, wbase + kWSig1);
+    mma_end();
+    wgmma_fence_regs<64>(d);
+    frag_store_relu64(sm.hs, d);
+    mma_begin();
+    mma_layer<16, 64>(d, a_hs, wbase + kWSig2);
+    mma_end();
+    wgmma_fence_regs<16>(d);
+    frag_stage<16, 16>(reinterpret_cast<float*>(sm.h1), d);   // h1 is written by the next round only
+    __syncthreads();
+    stage_read_row<16>(reinterpret_cast<const float*>(sm.h1), o);
     const float h0 = o[0];
     write_color_input(f, sm.cin, roff, vw, o);
-    const int K1 = f.color_in_width;
-    mma_round(sm, phase, [&] { issue_layer(tm + kColWork, a_cin, wbase + kWCol1, 64, K1); });
-    tmem_ld64(trow + kColWork, v);
-    store_relu64(sm.h1, roff, v);
-    mma_round(sm, phase, [&] { issue_layer(tm + kColWork, a_h1, wbase + w_col2(f.color_in_width), 64, 64); });
-    tmem_ld64(trow + kColWork, v);
-    store_relu64(sm.h2, roff, v);
-    mma_round(sm, phase, [&] { issue_layer(tm + kColWork, a_h2, wbase + w_col3(f.color_in_width), 16, 64); });
-    tmem_ld16(trow + kColWork, o);
+    mma_begin();
+    if (K1 == 48) mma_layer<64, 48>(d, a_cin, wbase + kWCol1);
+    else mma_layer<64, 32>(d, a_cin, wbase + kWCol1);
+    mma_end();
+    wgmma_fence_regs<64>(d);
+    frag_store_relu64(sm.h1, d);
+    mma_begin();
+    mma_layer<64, 64>(d, a_h1, wbase + w_col2(K1));
+    mma_end();
+    wgmma_fence_regs<64>(d);
+    frag_store_relu64(sm.h2, d);
+    mma_begin();
+    mma_layer<16, 64>(d, a_h2, wbase + w_col3(K1));
+    mma_end();
+    wgmma_fence_regs<16>(d);
+    frag_stage<16, 4>(reinterpret_cast<float*>(sm.gs), d);    // colour pre-activation 0..2; gs is written much later
+    __syncthreads();
+    stage_read_row<4>(reinterpret_cast<const float*>(sm.gs), o);
 
     // ---------------- backward ----------------
     {  // d(colour pre-activation) = d_rgb * rgb * (1 - rgb), cols 3..15 = 0
@@ -596,26 +591,41 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
           make_uint4(pack_bf16x2(d3[0], d3[1]), pack_bf16x2(d3[2], 0.f), 0u, 0u);
       *reinterpret_cast<uint4*>(sm.g3 + 1 * kAChunk + roff) = make_uint4(0u, 0u, 0u, 0u);
     }
-    mma_round(sm, phase, [&] {
-      issue_wgrad(tm + kColW3c, a_h2, a_g3, 16, have_acc);                   // dW3c^T += H2^T dO3
-      issue_dgrad(tm + kColWork, a_g3, wbase + w_col3(f.color_in_width), 64, 16);              // dH2 = dO3 W3c
-    });
-    tmem_ld64(trow + kColWork, v);
-    relu_backward_inplace64(sm.h2, roff, v);
-    mma_round(sm, phase, [&] {
-      issue_wgrad(tm + kColW2c, a_h2, a_h1, 64, have_acc);                   // dW2c += dH2^T H1
-      issue_dgrad(tm + kColWork, a_h2, wbase + w_col2(f.color_in_width), 64, 64);              // dH1 = dH2 W2c
-    });
-    tmem_ld64(trow + kColWork, v);
-    relu_backward_inplace64(sm.h1, roff, v);
-    mma_round(sm, phase, [&] {
-      issue_wgrad(tm + kColW1c, a_h1, a_cin, K1, have_acc);                  // dW1c += dH1^T Cin
-      issue_dgrad(tm + kColWork, a_h1, wbase + kWCol1, K1, 64);              // dCin = dH1 W1c
-    });
+    wgmma_fence_regs<8>(gw3c);
+    mma_begin();
+    issue_wgrad<16>(gw3c, a_h2, a_g3);                          // dW3c^T += H2^T dO3
+    issue_dgrad<64, 16>(d, a_g3, wbase + w_col3(K1));           // dH2 = dO3 W3c
+    mma_end();
+    wgmma_fence_regs<8>(gw3c);
+    wgmma_fence_regs<64>(d);
+    frag_relu_backward64(sm.h2, d);
+    wgmma_fence_regs<32>(gw2c);
+    mma_begin();
+    issue_wgrad<64>(gw2c, a_h2, a_h1);                          // dW2c += dH2^T H1
+    issue_dgrad<64, 64>(d, a_h2, wbase + w_col2(K1));           // dH1 = dH2 W2c
+    mma_end();
+    wgmma_fence_regs<32>(gw2c);
+    wgmma_fence_regs<64>(d);
+    frag_relu_backward64(sm.h1, d);
+    wgmma_fence_regs<24>(gw1c);
+    mma_begin();
+    if (K1 == 48) {
+      issue_wgrad<48>(gw1c, a_h1, a_cin);                       // dW1c += dH1^T Cin
+      issue_dgrad<48, 64>(d, a_h1, wbase + kWCol1);             // dCin = dH1 W1c
+    } else {
+      issue_wgrad<32>(gw1c, a_h1, a_cin);
+      issue_dgrad<32, 64>(d, a_h1, wbase + kWCol1);
+    }
+    mma_end();
+    wgmma_fence_regs<24>(gw1c);
+    wgmma_fence_regs<48>(d);
     {
+      // colour-input columns 16..47 (geometry features, camera embedding) staged in h2, free since the last round
       float dc[48];
-      tmem_ld32(trow + kColWork, dc);
-      if (K1 == 48) tmem_ld16(trow + kColWork + 32, dc + 32);
+      if (K1 == 48) frag_stage<48, 32, 16>(reinterpret_cast<float*>(sm.h2), d);
+      else frag_stage<32, 32, 16>(reinterpret_cast<float*>(sm.h2), d);
+      __syncthreads();
+      stage_read_row<32>(reinterpret_cast<const float*>(sm.h2), dc + 16);
       if (args.d_emb != nullptr && vw.cam >= 0) {  // d(camera embedding): colour-input features 31..30+E
         const int E = f.camera_embedding_dim;
 #pragma unroll
@@ -636,21 +646,28 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
       *reinterpret_cast<uint4*>(sm.gs + 1 * kAChunk + roff) = make_uint4(
           pack_bf16x2(dc[23], dc[24]), pack_bf16x2(dc[25], dc[26]), pack_bf16x2(dc[27], dc[28]), pack_bf16x2(dc[29], dc[30]));
     }
-    mma_round(sm, phase, [&] {
-      issue_wgrad(tm + kColW2s, a_hs, a_gs, 16, have_acc);                   // dW2s^T += Hs^T dOs
-      issue_dgrad(tm + kColWork, a_gs, wbase + kWSig2, 64, 16);              // dHs = dOs W2s
-    });
-    tmem_ld64(trow + kColWork, v);
-    relu_backward_inplace64(sm.hs, roff, v);
-    mma_round(sm, phase, [&] {
-      issue_wgrad(tm + kColW1s, a_hs, a_feat, 32, have_acc);                 // dW1s += dHs^T feat
-      issue_dgrad(tm + kColWork, a_hs, wbase + kWSig1, 32, 64);              // dFeat = dHs W1s
-    });
+    wgmma_fence_regs<8>(gw2s);
+    mma_begin();
+    issue_wgrad<16>(gw2s, a_hs, a_gs);                          // dW2s^T += Hs^T dOs
+    issue_dgrad<64, 16>(d, a_gs, wbase + kWSig2);               // dHs = dOs W2s
+    mma_end();
+    wgmma_fence_regs<8>(gw2s);
+    wgmma_fence_regs<64>(d);
+    frag_relu_backward64(sm.hs, d);
+    wgmma_fence_regs<16>(gw1s);
+    mma_begin();
+    issue_wgrad<32>(gw1s, a_hs, a_feat);                        // dW1s += dHs^T feat
+    issue_dgrad<32, 64>(d, a_hs, wbase + kWSig1);               // dFeat = dHs W1s
+    mma_end();
+    wgmma_fence_regs<16>(gw1s);
+    wgmma_fence_regs<32>(d);
     have_acc = true;
     {
       // d(composed features) -> global, level-major [16][N] float2 (coalesced here and in grid_scatter_kernel)
       float df[32];
-      tmem_ld32(trow + kColWork, df);
+      frag_stage<32, 32>(reinterpret_cast<float*>(sm.h1), d);   // h1 is free until the next tile's recompute
+      __syncthreads();
+      stage_read_row<32>(reinterpret_cast<const float*>(sm.h1), df);
       if (valid) {
 #pragma unroll
         for (int l = 0; l < 16; ++l) args.dfeat[(size_t)l * ns + i] = make_float2(df[2 * l], df[2 * l + 1]);
@@ -660,46 +677,17 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
 
   if (!weights_ready) mbar_wait(&sm.bar_w, 0);
   // ---------------- flush the weight-gradient accumulators ----------------
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
   if (have_acc && args.d_mlp != nullptr) {
-    const int lane = tid & 31, warp = tid >> 5;
-    const int m = warp * 16 + lane;  // M=64 accumulators: row m lives in lane m%16 of sub-partition m/16
     // Every CTA adds its 11 264 partial sums into the same 44 KB at the same moment (persistent CTAs finish together):
-    // rows that are contiguous per lane go out as 16-byte REDs, a quarter of the operations on those hot lines.
-    const bool v4ok = (reinterpret_cast<uintptr_t>(args.d_mlp) & 15u) == 0;
-    auto add_row = [&](float* dst, const float* a, int n) {   // n multiple of 4, dst 16-byte aligned when v4ok
-      if (v4ok) {
-#pragma unroll
-        for (int c = 0; c < 64; c += 4)
-          if (c < n) red_add_v4(dst + c, a[c], a[c + 1], a[c + 2], a[c + 3]);
-      } else {
-#pragma unroll
-        for (int c = 0; c < 64; ++c)
-          if (c < n) atomicAdd(dst + c, a[c]);
-      }
-    };
-    float acc[64];
-    tmem_ld32(trow + kColW1s, acc);
-    if (lane < 16) add_row(args.d_mlp + kGSig1 + m * 32, acc, 32);
-    tmem_ld16(trow + kColW2s, acc);
-    if (lane < 16)
-      for (int c = 0; c < 16; ++c) atomicAdd(args.d_mlp + kGSig2 + c * 64 + m, acc[c]);
-    const int K1 = f.color_in_width;
+    // the two adjacent columns a thread holds go out as one 8-byte RED where the destination row is contiguous.
+    const bool v2ok = (reinterpret_cast<uintptr_t>(args.d_mlp) & 7u) == 0;
     const int gcol2 = kGCol1 + 64 * K1, gcol3 = gcol2 + 4096;
-    tmem_ld32(trow + kColW1c, acc);
-    if (K1 == 48) tmem_ld16(trow + kColW1c + 32, acc + 32);
-    if (lane < 16) add_row(args.d_mlp + kGCol1 + m * K1, acc, K1);
-    tmem_ld64(trow + kColW2c, acc);
-    if (lane < 16) add_row(args.d_mlp + gcol2 + m * 64, acc, 64);
-    tmem_ld16(trow + kColW3c, acc);
-    if (lane < 16)
-      for (int c = 0; c < 16; ++c) atomicAdd(args.d_mlp + gcol3 + c * 64 + m, acc[c]);
+    flush_rows<16>(args.d_mlp + kGSig1, 32, gw1s, 32, v2ok);
+    flush_cols(args.d_mlp + kGSig2, gw2s);
+    flush_rows<24>(args.d_mlp + kGCol1, K1, gw1c, K1, v2ok);
+    flush_rows<32>(args.d_mlp + gcol2, 64, gw2c, 64, v2ok);
+    flush_cols(args.d_mlp + gcol3, gw3c);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tmem_dealloc(sm.tmem_base, kTmemCols);
 }
 
 }  // namespace hrf
@@ -762,7 +750,7 @@ int hrf_launch_scatter_v5(const hrf_field* f, const hrf_samples* s, const hrf_se
                           const int32_t* feat_index, int64_t grid_feat_stride, const void* workspace, int grid_first, int grid_count,
                           cudaStream_t st);   // scatter_v5.cu
 #ifndef HRF_SCATTER_DEFAULT
-#define HRF_SCATTER_DEFAULT 3   // measured on B200 (profiles/r2d_*, DESIGN.md section 3): v3 1.50 ms, v1 1.71, v2 1.86
+#define HRF_SCATTER_DEFAULT 5   // the fastest generation on the train bench on an H100 (DESIGN.md section 3.3)
 #endif
 
 extern "C" int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads,

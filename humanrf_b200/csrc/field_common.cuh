@@ -1,16 +1,16 @@
 // Device code shared by the forward and backward radiance-field kernels: sample loading,
 // multi-resolution hash-grid gathers (tcnn grid.h semantics), vector lerps
-// (tensor_composition.cu:30-45), shared-memory operand layouts for tcgen05.mma.
+// (tensor_composition.cu:30-45), shared-memory operand layouts for wgmma.
 #pragma once
 #include "common.cuh"
 
 namespace hrf {
 
-constexpr int kTile = 128;              // samples per CTA tile == UMMA M
+constexpr int kTile = 128;              // samples per CTA tile == threads per CTA == one warpgroup
 constexpr uint32_t kPrimeY = 2654435761u;  // tcnn coherent_prime_hash
 constexpr uint32_t kPrimeZ = 805459861u;
 
-// Byte offsets of the packed bf16 weight blob (UMMA K-major SWIZZLE_NONE core-matrix layout,
+// Byte offsets of the packed bf16 weight blob (K-major no-swizzle core-matrix layout,
 // element (n,k) of W[N,K] at ((k/8)*(N/8) + n/8)*128 + (n%8)*16 + (k%8)*2).
 constexpr uint32_t kWSig1 = 0;       // sigma  W1 [64,32]
 constexpr uint32_t kWSig2 = 4096;    // sigma  W2 [16,64]
@@ -378,21 +378,91 @@ __device__ __forceinline__ void encode_to_smem(const hrf_field& f, const Sample&
   }
 }
 
-// Issue one dense layer D[128,N] = A[128,K] * W[N,K]^T on the tensor cores (one thread).
-__device__ __forceinline__ void issue_layer(uint32_t tmem_d, uint32_t a_addr, uint32_t w_addr, int N, int K) {
-  const uint32_t idesc = make_idesc_bf16(kTile, N);
-  const uint32_t b_lbo = (uint32_t)(N >> 3) * 128u;
+// A 128-row tile is two m64 wgmma operands: rows 64h..64h+63 start 8 row groups of 128 bytes later per half.
+constexpr uint32_t kAHalf = 8u * 128u;
+
+// Issue one dense layer D[128,N] = A[128,K] * W[N,K]^T on the tensor cores (all 128 threads): rows 0-63 accumulate
+// into d[0, N/2), rows 64-127 into d[N/2, N).  kHalf = 0 | 1 issues the rows of that half only, into d[0, N/2).
+template <int N, int K, int kHalf = -1>
+__device__ __forceinline__ void mma_layer(float* d, uint32_t a_addr, uint32_t w_addr) {
+  constexpr uint32_t b_lbo = (uint32_t)(N >> 3) * 128u;
+#pragma unroll
   for (int k = 0; k < K / 16; ++k) {
-    const uint64_t ad = make_smem_desc(a_addr + (uint32_t)k * 2u * kAChunk, kAChunk, 128u);
     const uint64_t bd = make_smem_desc(w_addr + (uint32_t)k * 2u * b_lbo, b_lbo, 128u);
-    umma_bf16(tmem_d, ad, bd, idesc, k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (kHalf < 0 || h == kHalf)
+        wgmma_bf16<N>(d + (kHalf < 0 ? h * (N / 2) : 0),
+                      make_smem_desc(a_addr + h * kAHalf + (uint32_t)k * 2u * kAChunk, kAChunk, 128u), bd, k > 0 ? 1u : 0u);
+  }
+}
+
+// An MMA round: mma_begin() publishes the operand tiles written with ordinary stores to the tensor cores; after
+// mma_end() every MMA of the round has completed, so its operand tiles may be overwritten.
+__device__ __forceinline__ void mma_begin() {
+  fence_proxy_async_smem();
+  __syncthreads();
+  wgmma_fence();
+}
+__device__ __forceinline__ void mma_end() {
+  wgmma_commit();
+  wgmma_wait_all();
+  __syncthreads();
+}
+
+// Tile row and column of accumulator register q of this thread in half h of a 128-row result (see wgmma_bf16).
+__device__ __forceinline__ int frag_row(int h, int q) {
+  return 64 * h + 16 * (int)(threadIdx.x >> 5) + (int)((threadIdx.x & 31) >> 2) + 8 * ((q >> 1) & 1);
+}
+__device__ __forceinline__ int frag_col(int q) { return 8 * (q >> 2) + 2 * (int)(threadIdx.x & 3) + (q & 1); }
+
+// relu(D[128,64]) -> bf16 K-major tile (K = 64): the A operand of the next layer.  kHalf as in mma_layer.
+template <int kHalf = -1>
+__device__ __forceinline__ void frag_store_relu64(unsigned char* buf, const float* d) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int q = 0; q < 32; q += 2) {
+      if (kHalf >= 0 && h != kHalf) continue;
+      const int r = frag_row(h, q), c = frag_col(q), j = (kHalf < 0 ? h * 32 : 0) + q;
+      *reinterpret_cast<uint32_t*>(buf + (c >> 3) * kAChunk + a_row_off(r) + (c & 7) * 2) =
+          pack_bf16x2(fmaxf(d[j], 0.f), fmaxf(d[j + 1], 0.f));
+    }
+}
+
+// fp32 staging of columns [kC0, kC0 + kW) of D[128,N] (kW a power of two >= 4) so that thread r can read row r:
+// row-major, the 16-byte groups of a row XOR-swizzled by the row so that neither the fragment stores nor the row
+// reads pile onto a few banks.
+template <int kW>
+__device__ __forceinline__ int stage_off(int r, int c) {
+  constexpr int mask = (kW / 4 < 8 ? kW / 4 : 8) - 1;
+  return r * kW + ((((c >> 2) ^ (r & mask))) << 2) + (c & 3);
+}
+template <int N, int kW, int kC0 = 0>
+__device__ __forceinline__ void frag_stage(float* st, const float* d) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int q = 0; q < N / 2; q += 2) {
+      const int c = frag_col(q) - kC0;
+      if (c >= 0 && c < kW)
+        *reinterpret_cast<float2*>(st + stage_off<kW>(frag_row(h, q), c)) = make_float2(d[h * (N / 2) + q], d[h * (N / 2) + q + 1]);
+    }
+}
+template <int kW>
+__device__ __forceinline__ void stage_read_row(const float* st, float* v) {
+  const int r = threadIdx.x;
+#pragma unroll
+  for (int g = 0; g < kW / 4; ++g) {
+    const float4 x = *reinterpret_cast<const float4*>(st + stage_off<kW>(r, 4 * g));
+    v[4 * g] = x.x, v[4 * g + 1] = x.y, v[4 * g + 2] = x.z, v[4 * g + 3] = x.w;
   }
 }
 
 // Gradient of the TIME rows of `vectors` (grid xyz, tensor_composition.cu:49-52,109-111).  Every sample of a ray has the
 // same two rows and a batch holds a handful of frames (max_num_frames_per_batch, run_args.py:101): a whole scatter launch
-// adds into ~16 rows x 16 levels, i.e. a few 128-byte lines, and same-line REDs serialise in one L2 slice (measured: the
-// busiest slice at 69 % against 44 % on average; 1.42 -> 1.07 ms once these adds were combined, profiles/r2j_*, r2k_*).
+// adds into ~16 rows x 16 levels, i.e. a few 128-byte lines, and same-line REDs serialise in one L2 slice (which made the
+// scatter time depend on which frames a batch had drawn until these adds were combined).
 // The lanes of a warp walk about one ray: sum the lanes that hold the same row, one RED per distinct row and warp.
 // `key` identifies the row (0xffffffff: nothing to add), `addr` is the same for equal keys.  All 32 lanes must call.
 __device__ __forceinline__ void warp_combine_red2(uint32_t key, float* addr, float s0, float s1) {

@@ -1,9 +1,8 @@
-// Fused forward of the HumanRF radiance field for sm_100a:
-//   sample load -> 4 hash grids x 16 levels gather -> vector composition -> sigma MLP (tcgen05)
-//   -> truncated_exp density -> SH + colour MLP (tcgen05) -> sigmoid radiance.
-// One persistent CTA of 128 threads owns one 128-sample tile at a time; thread r owns sample r
-// (= row r of every MMA operand and TMEM lane r of every accumulator), so the whole
-// encode -> MLP chain stays in registers / shared memory / TMEM.
+// Fused forward of the HumanRF radiance field for sm_90a:
+//   sample load -> 4 hash grids x 16 levels gather -> vector composition -> sigma MLP (wgmma)
+//   -> truncated_exp density -> SH + colour MLP (wgmma) -> sigmoid radiance.
+// One persistent CTA of 128 threads (one warpgroup) owns one 128-sample tile at a time; thread r owns sample r
+// (= row r of every MMA operand), so the whole encode -> MLP chain stays in registers / shared memory.
 // Reference semantics: humanrf/scene_representation/humanrf.py:158-208,
 // decomposition4d.py:124-135, native/tensor_composition.cu:9-55.
 #include <stddef.h>
@@ -15,15 +14,13 @@ namespace hrf {
 
 
 // One activation buffer serves every layer: a layer's output tile is written over its input tile, which is safe
-// because each thread writes only after the tcgen05.commit barrier of the MMA that read the old tile.
+// because each thread writes only after the wgmma wait and the CTA barrier that follow the MMA that read the old tile.
+// The same buffer stages the fp32 outputs of the 16-wide layers so that every thread can read its row.
 // The weight blob comes LAST and only its used part is requested as dynamic shared memory (20 KB without camera
-// embeddings): 5 CTAs/SM then need 190 KB, which keeps the SM in the 196 KB shared-memory carve-out and leaves 60 KB
-// of L1 for the gathers (2 KB more per CTA tips it into the 228 KB carve-out and costs 20 % of the kernel time).
+// embeddings), so 5 CTAs/SM leave part of the 228 KB of shared memory and L1 to the L1 cache for the gathers.
 struct __align__(128) FwdSmem {
   unsigned char a[kTile * 64 * 2];    // A tile: K = 32 layout in the first 8 KB, or K = 64 layout (hidden activations)
   uint64_t bar_w;                     // weights landed
-  uint64_t bar_mma;                   // tcgen05.commit arrival
-  uint32_t tmem_base;
   // early-stop schedule: the current work item, published by thread 0
   int64_t item_start, item_end;
   int32_t item_ray, item_skip;
@@ -36,55 +33,30 @@ __device__ __forceinline__ float warp_sum_fwd(float v) {
   return v;
 }
 
-template <int N>
-__device__ __forceinline__ void tmem_load_row(uint32_t taddr, float* v) {
-  if constexpr (N == 64) tmem_ld64(taddr, v);
-  else if constexpr (N == 32) tmem_ld32(taddr, v);
-  else tmem_ld16(taddr, v);
-}
-
-// One dense layer for the CTA's tile; every thread ends up with its row's N outputs in v[].
-// kSimt == true is the fp32 CUDA-core debug path (tests only).
-template <bool kSimt, int N, int K>
-__device__ __forceinline__ void run_layer(FwdSmem& sm, const unsigned char* abuf, uint32_t woff, uint32_t& phase,
-                                          float* v) {
+// fp32 CUDA-core version of one dense layer (the debug path, tests only): every thread computes its row's N outputs.
+template <int N, int K>
+__device__ __forceinline__ void simt_layer(FwdSmem& sm, const unsigned char* abuf, uint32_t woff, float* v) {
   const int tid = threadIdx.x;
-  if constexpr (!kSimt) {
-    tc_fence_before();
-    fence_proxy_async_smem();
-    __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      issue_layer(sm.tmem_base, smem_u32(abuf), smem_u32(sm.w + woff), N, K);
-      umma_commit(&sm.bar_mma);
-    }
-    mbar_wait(&sm.bar_mma, phase);
-    phase ^= 1u;
-    tc_fence_after();
-    const uint32_t taddr = sm.tmem_base + ((uint32_t)(tid & ~31) << 16);
-    tmem_load_row<N>(taddr, v);
-  } else {
-    __syncthreads();
-    const uint32_t roff = a_row_off(tid);
-    float in[K];
+  __syncthreads();
+  const uint32_t roff = a_row_off(tid);
+  float in[K];
+#pragma unroll
+  for (int k = 0; k < K; k += 2) {
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(abuf + (k >> 3) * kAChunk + roff + (k & 7) * 2);
+    in[k] = bf16_lo(u), in[k + 1] = bf16_hi(u);
+  }
+#pragma unroll 4
+  for (int n = 0; n < N; ++n) {
+    float acc = 0.f;
 #pragma unroll
     for (int k = 0; k < K; k += 2) {
-      const uint32_t u = *reinterpret_cast<const uint32_t*>(abuf + (k >> 3) * kAChunk + roff + (k & 7) * 2);
-      in[k] = bf16_lo(u), in[k + 1] = bf16_hi(u);
+      const uint32_t u = *reinterpret_cast<const uint32_t*>(sm.w + woff + w_off(n, k, N));
+      acc = __fmaf_rn(in[k], bf16_lo(u), acc);
+      acc = __fmaf_rn(in[k + 1], bf16_hi(u), acc);
     }
-#pragma unroll 4
-    for (int n = 0; n < N; ++n) {
-      float acc = 0.f;
-#pragma unroll
-      for (int k = 0; k < K; k += 2) {
-        const uint32_t u = *reinterpret_cast<const uint32_t*>(sm.w + woff + w_off(n, k, N));
-        acc = __fmaf_rn(in[k], bf16_lo(u), acc);
-        acc = __fmaf_rn(in[k + 1], bf16_hi(u), acc);
-      }
-      v[n] = acc;
-    }
-    __syncthreads();
+    v[n] = acc;
   }
+  __syncthreads();
 }
 
 // relu -> bf16 -> K-major A tile with K = 64
@@ -98,6 +70,50 @@ __device__ __forceinline__ void store_hidden(unsigned char* hbuf, int row, const
     q.z = pack_bf16x2(fmaxf(v[kg * 8 + 4], 0.f), fmaxf(v[kg * 8 + 5], 0.f));
     q.w = pack_bf16x2(fmaxf(v[kg * 8 + 6], 0.f), fmaxf(v[kg * 8 + 7], 0.f));
     *reinterpret_cast<uint4*>(hbuf + kg * kAChunk + roff) = q;
+  }
+}
+
+// One dense layer with 16 outputs; every thread ends up with its row's outputs in v[].  kSimt == true is the fp32
+// CUDA-core debug path (tests only).  On return the A tile is free for the next operands.
+template <bool kSimt, int K>
+__device__ __forceinline__ void run_layer16(FwdSmem& sm, uint32_t woff, float* v) {
+  if constexpr (!kSimt) {
+    float d[16];
+    mma_begin();
+    mma_layer<16, K>(d, smem_u32(sm.a), smem_u32(sm.w + woff));
+    mma_end();
+    wgmma_fence_regs<16>(d);
+    float* st = reinterpret_cast<float*>(sm.a);
+    frag_stage<16, 16>(st, d);
+    __syncthreads();
+    stage_read_row<16>(st, v);
+    __syncthreads();
+  } else {
+    simt_layer<16, K>(sm, sm.a, woff, v);
+  }
+}
+
+// One hidden layer with 64 outputs: relu -> bf16 written over the A tile, the K = 64 operand of the next layer.
+// One 64-row half at a time: the halves read and write disjoint rows of the tile, and 32 accumulators a thread
+// instead of 64 keep the kernel within the 96 registers of 5 CTAs per SM without spilling.
+template <bool kSimt, int K>
+__device__ __forceinline__ void run_hidden(FwdSmem& sm, uint32_t woff) {
+  if constexpr (!kSimt) {
+    float d[32];
+    mma_begin();
+    mma_layer<64, K, 0>(d, smem_u32(sm.a), smem_u32(sm.w + woff));
+    mma_end();
+    wgmma_fence_regs<32>(d);
+    frag_store_relu64<0>(sm.a, d);
+    mma_begin();
+    mma_layer<64, K, 1>(d, smem_u32(sm.a), smem_u32(sm.w + woff));
+    mma_end();
+    wgmma_fence_regs<32>(d);
+    frag_store_relu64<1>(sm.a, d);
+  } else {
+    float v[64];
+    simt_layer<64, K>(sm, sm.a, woff, v);
+    store_hidden(sm.a, threadIdx.x, v);
   }
 }
 
@@ -116,27 +132,17 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
   const int tid = threadIdx.x;
   const hrf_field& f = args.f;
 
-  // ---- one-time CTA setup: barriers, TMEM, weights via TMA bulk copy -------------------
+  // ---- one-time CTA setup: barrier, weights via TMA bulk copy -------------------
   if (tid == 0) {
     mbar_init(&sm.bar_w, 1);
-    mbar_init(&sm.bar_mma, 1);
     fence_mbar_init();
   }
-  if constexpr (!kSimt) {
-    if (tid < 32) {
-      tmem_alloc(&sm.tmem_base, 64);
-      tmem_relinquish();
-    }
-    tc_fence_before();
-  }
   __syncthreads();
-  if constexpr (!kSimt) tc_fence_after();
   if (tid == 0) {
     mbar_arrive_expect_tx(&sm.bar_w, w_blob_bytes(f.color_in_width));
     tma_load_1d(sm.w, f.mlp_blob, w_blob_bytes(f.color_in_width), &sm.bar_w);
   }
   bool weights_ready = false;
-  uint32_t phase = 0;
 
   const int64_t n = live_samples(args.s);
   const int64_t n_stride = args.s.num_samples;   // row length of the level-major [64][N] output
@@ -211,11 +217,9 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
     }
 
     // ---- sigma net: 32 -> 64 (ReLU) -> 16 ------------------------------------------------
-    float v[64];
-    run_layer<kSimt, 64, 32>(sm, sm.a, kWSig1, phase, v);
-    store_hidden(sm.a, tid, v);
+    run_hidden<kSimt, 32>(sm, kWSig1);
     float o[16];
-    run_layer<kSimt, 16, 64>(sm, sm.a, kWSig2, phase, o);
+    run_layer16<kSimt, 64>(sm, kWSig2, o);
     // humanrf.py:184 : density = truncated_exp(h[...,0]) * density_scale  (exp in fp32)
     const float sigma = __expf(o[0]) * f.density_scale;
     if (es) {  // publish this item's optical depth
@@ -236,12 +240,10 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
 
     // ---- colour net: [SH16 | geo15 | 1.0] -> 64 (ReLU) -> 64 (ReLU) -> 16 -> sigmoid[:3] ----
     write_color_input(f, sm.a, a_row_off(tid), load_view(f, args.s, valid ? i : n, n), o);
-    if (f.color_in_width == 48) run_layer<kSimt, 64, 48>(sm, sm.a, kWCol1, phase, v);
-    else run_layer<kSimt, 64, 32>(sm, sm.a, kWCol1, phase, v);
-    store_hidden(sm.a, tid, v);
-    run_layer<kSimt, 64, 64>(sm, sm.a, w_col2(f.color_in_width), phase, v);
-    store_hidden(sm.a, tid, v);
-    run_layer<kSimt, 16, 64>(sm, sm.a, w_col3(f.color_in_width), phase, o);
+    if (f.color_in_width == 48) run_hidden<kSimt, 48>(sm, kWCol1);
+    else run_hidden<kSimt, 32>(sm, kWCol1);
+    run_hidden<kSimt, 64>(sm, w_col2(f.color_in_width));
+    run_layer16<kSimt, 64>(sm, w_col3(f.color_in_width), o);
     const float c0 = 1.f / (1.f + __expf(-o[0])), c1 = 1.f / (1.f + __expf(-o[1])), c2 = 1.f / (1.f + __expf(-o[2]));
     if (valid && args.rgb != nullptr) {
       float* rp = args.rgb + 3 * i;
@@ -312,11 +314,6 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
 
   // ---- teardown ---------------------------------------------------------------------------
   if (!weights_ready) mbar_wait(&sm.bar_w, 0);  // never leave a bulk copy in flight
-  if constexpr (!kSimt) {
-    tc_fence_before();
-    __syncthreads();
-    if (tid < 32) tmem_dealloc(sm.tmem_base, 64);
-  }
 }
 
 }  // namespace hrf
@@ -326,8 +323,9 @@ using namespace hrf;
 static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t st, bool persistent_full) {
   const int64_t tiles = (a.s.num_samples + kTile - 1) / kTile;
   const int smem = (int)(offsetof(FwdSmem, w) + w_blob_bytes(a.f.color_in_width)) + 128;
-  // CTAs per SM, measured on B200 on the bench batch with 4 levels unrolled: 4 (118 regs) 1.291 ms, 5 (96 regs)
-  // 1.265 ms, 6 (80 regs, spills) 1.475 ms.  HRF_FWD_CTAS overrides for experiments (4 and 6 keep the 4-level unroll).
+  // CTAs per SM, measured on an H100 (400 W) on the render bench (scripts/tuning_ab.sh): 5 (96 regs) 1.38 ms per step,
+  // 4 (4-level unroll) 1.61 ms, 6 (80 regs, spills) 1.99 ms.  HRF_FWD_CTAS overrides for experiments (4 keeps the 4-level
+  // unroll).
   static const int ctas_per_sm = [] {
     const char* e = getenv("HRF_FWD_CTAS");
     const int v = e ? atoi(e) : 5;
@@ -343,10 +341,9 @@ static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t s
     kernel<<<grid, kTile, smem, st>>>(a);
     return 0;
   };
-  // Levels unrolled in the encode loop (HRF_FWD_UNROLL = 1 | 2 | 4).  Measured on B200 on the bench batch
-  // (profiles/r1_fwd_unroll.txt): 4 levels -> 1.283 ms (7 344 SASS instructions = 117 KB, ncu: no-instruction stalls
-  // 2.3 per issue), 2 -> 1.145 ms, 1 -> 1.034 ms (3 336 instructions): the instruction cache, not gather ILP, was
-  // the limiter.  Default 1.
+  // Levels unrolled in the encode loop (HRF_FWD_UNROLL = 1 | 2 | 4).  The 4-level loop is over twice the code of the
+  // 1-level one, and the instruction cache, not gather ILP, limits it; on an H100 (400 W, render bench) 1 level takes
+  // 1.38 ms per step, 2 and 4 levels 1.40 ms.  Default 1.
   static const int unroll = [] { const char* e = getenv("HRF_FWD_UNROLL"); const int v = e ? atoi(e) : 1; return (v == 2 || v == 4) ? v : 1; }();
   int rc;
   if (a.comp.ray_offsets != nullptr && a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true, true>);

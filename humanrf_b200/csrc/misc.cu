@@ -1,4 +1,4 @@
-// Error plumbing, device info, fused Adam, bf16 cast and the tcgen05 descriptor self-test.
+// Error plumbing, device info, fused Adam, bf16 cast and the wgmma descriptor self-test.
 #include <mutex>
 
 #include "field_common.cuh"
@@ -20,7 +20,7 @@ int sm_count() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      return 148;
+      return 132;   // H100 SXM
   }
   return cached;
 }
@@ -52,8 +52,9 @@ __global__ void cast_bf16_kernel(const float* __restrict__ s, __nv_bfloat16* __r
 }
 
 // ---------------------------------------------------------------------------------------
-// tcgen05 descriptor self-test: D[M,N] = A[M,K] * B[N,K]^T with caller-chosen placement
-// strides and descriptor fields.
+// wgmma descriptor self-test: D[M,N] = A[M,K] * B[N,K]^T with caller-chosen placement
+// strides and descriptor fields.  M = 128 runs as two m64 halves whose A operands start
+// 8 row groups (8 * a_mstride bytes) apart, as in the field kernels.
 // ---------------------------------------------------------------------------------------
 struct SelfTestArgs {
   const __nv_bfloat16* a;
@@ -65,22 +66,40 @@ struct SelfTestArgs {
   int mn_major;
 };
 
+template <int N, int kTransA, int kTransB>
+__device__ __forceinline__ void selftest_mma(const SelfTestArgs& t, uint32_t sa, uint32_t sb) {
+  float d[N] = {};
+  wgmma_fence();
+  for (int k = 0; k < t.k / 16; ++k) {
+    const uint64_t bd = make_smem_desc(sb + (uint32_t)k * 2u * t.b_kstride, t.b_lbo, t.b_sbo);
+    const uint32_t a0 = sa + (uint32_t)k * 2u * t.a_kstride;
+    wgmma_bf16<N, kTransA, kTransB>(d, make_smem_desc(a0, t.a_lbo, t.a_sbo), bd, k > 0);
+    if (t.m == 128) wgmma_bf16<N, kTransA, kTransB>(d + N / 2, make_smem_desc(a0 + 8u * t.a_mstride, t.a_lbo, t.a_sbo), bd, k > 0);
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  wgmma_fence_regs<N>(d);
+  for (int h = 0; h < t.m / 64; ++h)
+#pragma unroll
+    for (int q = 0; q < N / 2; ++q) t.d[(int64_t)frag_row(h, q) * t.n + frag_col(q)] = d[h * (N / 2) + q];
+}
+
+template <int N>
+__device__ __forceinline__ void selftest_mma_n(const SelfTestArgs& t, uint32_t sa, uint32_t sb) {
+  switch (t.mn_major) {
+    case 0: selftest_mma<N, 0, 0>(t, sa, sb); break;
+    case 1: selftest_mma<N, 1, 0>(t, sa, sb); break;
+    case 2: selftest_mma<N, 0, 1>(t, sa, sb); break;
+    default: selftest_mma<N, 1, 1>(t, sa, sb); break;
+  }
+}
+
 __global__ void __launch_bounds__(128, 1) selftest_umma_kernel(const SelfTestArgs t) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   unsigned char* sa = base;            // up to 64 KB
   unsigned char* sb = base + 65536;    // up to 64 KB
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_base;
   const int tid = threadIdx.x;
-  if (tid == 0) {
-    mbar_init(&bar, 1);
-    fence_mbar_init();
-  }
-  if (tid < 32) {
-    tmem_alloc(&tmem_base, 256);
-    tmem_relinquish();
-  }
   // operand placement
   for (int e = tid; e < t.m * t.k; e += blockDim.x) {
     const int r = e / t.k, k = e % t.k;
@@ -100,35 +119,14 @@ __global__ void __launch_bounds__(128, 1) selftest_umma_kernel(const SelfTestArg
       off = (uint32_t)(r >> 3) * t.b_nstride + (uint32_t)(k >> 3) * t.b_kstride + (uint32_t)(k & 7) * 16u + (uint32_t)(r & 7) * 2u;
     *reinterpret_cast<__nv_bfloat16*>(sb + off) = t.b[e];
   }
-  tc_fence_before();
   fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  if (tid == 0) {
-    const uint32_t idesc = make_idesc_bf16(t.m, t.n, t.mn_major & 1, (t.mn_major >> 1) & 1);
-    for (int k = 0; k < t.k / 16; ++k) {
-      const uint64_t ad = make_smem_desc(smem_u32(sa) + (uint32_t)k * 2u * t.a_kstride, t.a_lbo, t.a_sbo);
-      const uint64_t bd = make_smem_desc(smem_u32(sb) + (uint32_t)k * 2u * t.b_kstride, t.b_lbo, t.b_sbo);
-      umma_bf16(tmem_base, ad, bd, idesc, k > 0);
-    }
-    umma_commit(&bar);
+  switch (t.n) {
+    case 16: selftest_mma_n<16>(t, smem_u32(sa), smem_u32(sb)); break;
+    case 32: selftest_mma_n<32>(t, smem_u32(sa), smem_u32(sb)); break;
+    case 48: selftest_mma_n<48>(t, smem_u32(sa), smem_u32(sb)); break;
+    default: selftest_mma_n<64>(t, smem_u32(sa), smem_u32(sb)); break;
   }
-  mbar_wait(&bar, 0);
-  tc_fence_after();
-  // read back: lane L of warp w holds row: M=128 -> row = 32w+L ; M=64 -> rows live in lanes 0..15 of each warp
-  const int lane = tid & 31, warp = tid >> 5;
-  int row = -1;
-  if (t.m == 128) row = tid;
-  else if (lane < 16) row = warp * 16 + lane;
-  for (int c0 = 0; c0 < t.n; c0 += 16) {
-    float v[16];
-    tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0, v);
-    if (row >= 0)
-      for (int j = 0; j < 16; ++j) t.d[(int64_t)row * t.n + c0 + j] = v[j];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (tid < 32) tmem_dealloc(tmem_base, 256);
 }
 
 }  // namespace hrf
@@ -174,7 +172,7 @@ extern "C" int hrf_selftest_umma(const void* a_bf16, const void* b_bf16, float* 
                                  uint32_t a_lbo, uint32_t a_sbo, uint32_t b_lbo, uint32_t b_sbo, int mn_major,
                                  void* stream) {
   HRF_REQUIRE(m == 64 || m == 128, "M must be 64 or 128");
-  HRF_REQUIRE(n % 16 == 0 && n >= 16 && n <= 256 && k % 16 == 0 && k >= 16 && k <= 128, "bad N/K");
+  HRF_REQUIRE(n % 16 == 0 && n >= 16 && n <= 64 && k % 16 == 0 && k >= 16 && k <= 128, "N must be 16..64, K 16..128");
   SelfTestArgs t{(const __nv_bfloat16*)a_bf16, (const __nv_bfloat16*)b_bf16, d, m, n, k, a_kstride, a_mstride,
                  b_kstride, b_nstride, a_lbo, a_sbo, b_lbo, b_sbo, mn_major};
   const int smem = 2 * 65536 + 1024;

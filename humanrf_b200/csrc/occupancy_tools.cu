@@ -102,7 +102,7 @@ extern "C" int hrf_occupancy_from_masks(const uint8_t* masks, const float* proje
   CarveArgs a{masks, projection_matrices, landscape_modes, camera_coverage_threshold, num_cameras, grid_resolution, width,
               height, occupancy_grid};
   const int64_t n = (int64_t)grid_resolution * grid_resolution * grid_resolution;
-  // 4 strided chunks of 256 voxels per CTA (measured at G=256, 24 cameras: 1 -> 0.524, 4 -> 0.519, 16 -> 0.588, one wave -> 0.651 ms):
+  // 4 strided chunks of 256 voxels per CTA (HRF_CARVE_CHUNKS overrides, scripts/carve_probe.py compares settings):
   // voxels differ a lot in cost (early exits), so many short CTAs balance better than a one-wave persistent grid
   const int64_t want = (n + 255) / 256, floor_ = (int64_t)sm_count() * 8;
   static const int chunks = [] { const char* e = getenv("HRF_CARVE_CHUNKS"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 4; }();

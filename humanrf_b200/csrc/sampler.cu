@@ -1,5 +1,5 @@
-// Ray generation, AABB slab test, occupancy march and sample generation for sm_100a.
-// Replaces actorshq/dataset/native/{occupancy_grid.cu, ray_sampler.cu}.  B200-first choices:
+// Ray generation, AABB slab test, occupancy march and sample generation for sm_90a.
+// Replaces actorshq/dataset/native/{occupancy_grid.cu, ray_sampler.cu}.  Design choices:
 //   * occupancy volumes are bit-packed (G^3/8 bytes: 2 MB at G=256, L2-resident) and the
 //     texture unit's 1.8 fixed-point trilinear ">0" test is emulated exactly in integer math;
 //   * one WARP per ray marches 32 steps at a time (ballot + ffs) instead of one divergent
@@ -32,7 +32,8 @@ __device__ __forceinline__ int fix8(float p, float G) {
   const float xb = __fsub_rn(__fmul_rn(p, G), 0.5f);
   return (int)floorf(__fadd_rn(__fmul_rn(xb, 256.f), 0.5f));
 }
-// Per-corner weight of the hardware filter (fitted on a B200 texture unit, see oracle/sampler.py):
+// Per-corner weight of the hardware filter (fitted on a texture unit, see oracle/sampler.py; tests/test_texture_probe_gpu.py
+// checks it against the texture unit of the GPU it runs on):
 // W = (((wx*wz + 128) >> 8) * wy + 128) >> 8 in 1/256 units; the sample is "> 0" iff an occupied
 // corner has W >= 1.
 __device__ __forceinline__ bool occ_lookup(const uint32_t* __restrict__ bits, int G, float x, float y, float z) {

@@ -1,9 +1,8 @@
 // Table / vector gradient scatter, second generation (replaces tcnn kernel_grid_backward + compose_tensors_backward,
 // tensor_composition.cu:57-118, like grid_scatter_staged_kernel in field_bwd.cu, which it supersedes as the default).
 //
-// Why: ncu on the staged kernel (profiles/r2a_ncu_full_bwd_raw.csv) shows 778 M warp instructions for 60.8 M
-// (sample, level, grid) items -- 2.7x what converged code needs -- and RED instructions issued with 8.6 of 32 lanes
-// active: the run-length logic ("new cell? shift the shared corners, flush the ones that leave") is a data-dependent
+// Why: the staged kernel issues several times the warp instructions converged code needs per (sample, level, grid)
+// item, and its RED instructions run with about a quarter of the lanes active: the run-length logic ("new cell? shift the shared corners, flush the ones that leave") is a data-dependent
 // branch per lane, and at the middle levels some lane of the warp takes it at almost every step.
 //
 // Here the per-sample step is STRAIGHT-LINE code.  The 8 accumulator slots of a thread are not indexed by corner
@@ -318,7 +317,7 @@ int hrf_launch_scatter_v2(const hrf_field* f, const hrf_samples* s, const hrf_se
   const int64_t blocks = (s->num_samples + kV2Samples - 1) / kV2Samples;
   const dim3 grid((unsigned)blocks, (HRF_N_LEVELS / kV2Levels) * grid_count);
   const int smem = (int)sizeof(V2Smem);
-  // CTAs per SM: 6 (80 registers, a few spilled words) or 5 (96 registers, no spills): HRF_SCATTER_CTAS, A/B on B200 in DESIGN.md
+  // CTAs per SM: 6 (80 registers, a few spilled words) or 5 (96 registers, no spills): HRF_SCATTER_CTAS
   const int ctas = [] { const char* e = getenv("HRF_SCATTER_CTAS"); return (e && e[0] == '5') ? 5 : 6; }();
   if (grid_feat_bf16 != nullptr) {
     if (ctas == 5) grid_scatter_v2_kernel<false, 5><<<grid, kV2Threads, smem, st>>>(a);

@@ -1,10 +1,9 @@
 // Table / vector gradient scatter, third generation (replaces tcnn kernel_grid_backward + compose_tensors_backward,
 // tensor_composition.cu:57-118).  Same algorithm as scatter_v2.cu (parity-slot accumulators: the shared-corner carry of the
-// run-length scheme as straight-line code), restructured around what ncu showed on v2 (profiles/r2c_*): 28 % issue-slot
-// utilisation, 54 % of the stall samples on long-scoreboard waits spread over (a) the shared-memory staging of every
-// level behind block-wide barriers, (b) the two vector-row loads of every step, which miss the 28 KB of L1 left beside
-// 200 KB of shared memory because `vectors` is [axis][row][32 features]: the 8 bytes one (level, row) needs sit in a
-// 128-byte line of their own.
+// run-length scheme as straight-line code), restructured around where v2 stalled (low issue-slot use, mostly
+// long-scoreboard waits) spread over (a) the shared-memory staging of every level behind block-wide barriers, (b) the
+// two vector-row loads of every step, which miss the small L1 left beside the shared memory because `vectors` is
+// [axis][row][32 features]: the 8 bytes one (level, row) needs sit in a 128-byte line of their own.
 //   * staging is WARP-private: a warp stages the 256 samples its own lanes walk (coalesced loads, __syncwarp), so the
 //     warps of a CTA no longer stop together at every level and one warp's staging latency hides behind the others' steps;
 //   * a CTA covers 8 levels (not 4) of its samples: positions / segment ids are staged half as often;
@@ -116,7 +115,7 @@ __device__ __forceinline__ void scatter_levels(const ScatterV3Args& a, V3Smem& s
   const int row = tid * kV3Row;
   const int cnt = min(max(valid - tid * kV3Chunk, 0), kV3Chunk);
   // columns of this lane's 8 staging slots inside egrid: the same for every level, fetched once (per level they would
-  // be a second, dependent global load in front of every staged value: 19 % of the stall samples of the first v3 cut)
+  // be a second, dependent global load in front of every staged value, a visible share of the stalls of the first v3 cut)
   int32_t col8[kV3Chunk];        // (a launch covers < 2^31 samples)
   if (!kGather) {
     const int w0 = (tid & ~31) * kV3Chunk, lane = tid & 31;

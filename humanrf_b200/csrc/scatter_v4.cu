@@ -1,8 +1,7 @@
 // Table / vector gradient scatter, fourth generation (replaces tcnn kernel_grid_backward + compose_tensors_backward,
 // tensor_composition.cu:57-118).  Same arithmetic as scatter_v3.cu; the change is OCCUPANCY.
 //
-// ncu on v3 (profiles/r2e_*, r2g_*): 39 % of the issue slots, 0.7 eligible warps per scheduler and cycle, 30 % of the warp
-// slots -- 96 registers per thread (8 table indices + 16 accumulators + run state) allow 5 CTAs x 4 warps per SM, and
+// v3 looks latency-bound (few eligible warps per scheduler and cycle): 96 registers per thread (8 table indices + 16 accumulators + run state) allow 5 CTAs x 4 warps per SM, and
 // three attempts to hide the remaining latencies inside a thread (prefetching, cp.async double buffering, shared-memory
 // descriptors) changed nothing.  Here the 8 parity slots of a sample chunk are split over TWO threads: warps 0-3 of a
 // 256-thread CTA own the slots whose third-axis vertex is even, warps 4-7 the odd ones (4 indices + 8 accumulators each).

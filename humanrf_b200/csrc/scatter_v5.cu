@@ -2,10 +2,8 @@
 // tensor_composition.cu:57-118).  Same arithmetic as scatter_v3.cu / scatter_v4.cu; the change is what ONE RED
 // INSTRUCTION carries to the L2.
 //
-// ncu on v3 and v4 (profiles/r2g_*, r2i_*): two kernels with very different SM-side pictures (39 % / 49 % of the issue
-// slots, 20 / 32 warps per SM) take the same 1.47 ms, and both send 145 M RED requests of ONE sector each to the L2
-// (lts__t_tag_requests: 44 % on average, 69 % on the busiest slice, half of the requests crossing the die fabric).  A
-// thread owns all vertices of its sample, so the 32 lanes of a RED instruction address 32 unrelated cells: one request
+// v3 and v4, two kernels with very different SM-side pictures (issue slots, warps per SM), take about the same time,
+// and both send one RED request of ONE sector per lane to the L2.  A thread owns all vertices of its sample, so the 32 lanes of a RED instruction address 32 unrelated cells: one request
 // per lane.  But the two vertices of a cell that differ in the FIRST axis are neighbours in the table (tcnn's hash
 // multiplies the first axis by 1; a dense level is x-major): 15 times out of 16 they lie in the same 128-byte line.
 // Here the 8 parity slots of a sample chunk are split over the two lanes of a LANE PAIR by the parity of the first-axis

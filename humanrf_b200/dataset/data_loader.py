@@ -4,7 +4,8 @@ actorshq/dataset/data_loader.py: same constructor arguments / enums, iterator pr
 ``pause_replacing`` / ``continue_replacing`` (:525-529), ``num_batches_per_full_image``,
 ``num_camera_frame_pairs``, ``render_sequence``, ``cameras``, ``dataset``, ``resolution``, ``aabb``.
 
-What is different by design (B200: 180 GB of HBM, no reason to bounce pixels through the host):
+What is different by design (the reference's default pool of 200 images, RGBA + light mask, takes 12 GB of the GPU's
+80 GB at full resolution and 0.8 GB at 4x downscale: no reason to bounce pixels through the host):
 * the uint8 RGBA pool and the light-bloom mask live ON THE GPU; the sampler gathers ground-truth colours inside
   its kernels (the reference keeps the pool on the CPU and does ``rgba.index({ray_indices.cpu()}) -> .cuda()`` per
   call, ray_sampler.cu:262);

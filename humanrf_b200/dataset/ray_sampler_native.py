@@ -4,7 +4,7 @@ actorshq/dataset/native/ray_sampler.cu:327-333 with the identical 15-argument si
 
 As in the reference, ``rgba`` (uint8 [P,4]) and ``light_mask`` (bool [P]) may live on the CPU
 (CHECK_CONTIGUITY_AND_DEVICE(..., kCPU), :215-216); then the per-ray gathers are done the
-reference's way (index on the host, one H2D copy, :254-257,262).  B200-first extension: when they
+reference's way (index on the host, one H2D copy, :254-257,262).  Extension: when they
 are CUDA tensors (a GPU-resident image pool, SURVEY 8f-1) the gathers happen inside the sampler
 kernels and nothing touches the host.  The whole call performs ONE host read (two counters) to
 size its outputs; the reference needs >= 5 implicit syncs.

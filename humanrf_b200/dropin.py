@@ -1,4 +1,4 @@
-"""Makes the reference's own import paths resolve to the B200 implementation, so `humanrf/run.py` and
+"""Makes the reference's own import paths resolve to this implementation, so `humanrf/run.py` and
 `humanrf/trainer.py` run unchanged (SURVEY 8b):
 
     import humanrf_b200.dropin; humanrf_b200.dropin.install()      # before importing humanrf.run / humanrf.trainer

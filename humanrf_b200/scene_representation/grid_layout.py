@@ -48,7 +48,7 @@ class GridLayout:
         return self.n_entries * N_FEATURES_PER_LEVEL
 
 
-# ---- packed bf16 MLP blob (UMMA K-major SWIZZLE_NONE core-matrix layout, csrc/field_common.cuh) ----
+# ---- packed bf16 MLP blob (wgmma K-major no-swizzle core-matrix layout, csrc/field_common.cuh) ----
 MLP_SIGMA_PARAMS = 64 * 32 + 16 * 64          # 3072  (tcnn FullyFusedMLP, output padded to 16)
 MLP_BLOB_ELEMS = 22528 // 2
 

@@ -1,4 +1,4 @@
-"""HumanRF scene representation backed by the fused sm_100a kernels.
+"""HumanRF scene representation backed by the fused sm_90a kernels.
 
 Drop-in for humanrf/scene_representation/humanrf.py:14-220 (+ decomposition4d.py:41-135): same
 constructor kwargs, ``density`` / ``forward`` / ``get_params``, same state-dict keys
@@ -11,8 +11,8 @@ constructor kwargs, ``density`` / ``forward`` / ``get_params``, same state-dict 
 so checkpoints written by the reference trainer load unchanged (trainer.py:528-620).  What is
 different by design: tables are read by the kernels from bf16 shadow copies of the fp32 master
 parameters (refreshed whenever a parameter's version changes); all segments stay resident in
-HBM (the reference off-loads idle segments to the host, humanrf.py:169-179 -- pointless with
-180 GB); encode -> MLP runs in one kernel instead of 4 tcnn encodings + compose + 2 tcnn nets.
+HBM (the reference off-loads idle segments to the host, humanrf.py:169-179; a 50-frame segment with its
+optimiser state takes about 0.5 GB of the GPU's 80 GB); encode -> MLP runs in one kernel instead of 4 tcnn encodings + compose + 2 tcnn nets.
 """
 from __future__ import annotations
 
@@ -45,7 +45,7 @@ class Decomposition4D(torch.nn.Module):
                  ngp_finest_resolution=2048, vectors_finest_resolution=2048):
         super().__init__()
         if ngp_n_levels != 16 or ngp_n_features_per_level != 2:
-            raise NotImplementedError("the sm_100a kernels are specialised for n_levels=16, n_features_per_level=2")
+            raise NotImplementedError("the sm_90a kernels are specialised for n_levels=16, n_features_per_level=2")
         self.layout = GridLayout(ngp_log2_hashmap_size, ngp_n_levels, ngp_base_resolution, ngp_finest_resolution)
         feature_size = ngp_n_levels * ngp_n_features_per_level
         self.vectors = torch.nn.Parameter(torch.randn((4, vectors_finest_resolution, feature_size)) * 0.1)  # :76-78
@@ -74,7 +74,7 @@ class HumanRF(torch.nn.Module):
         super().__init__()
         if (n_neurons, geometry_feature_dim, n_hidden_layers_density, n_hidden_layers_color, sh_degree) != (64, 15, 1, 2, 4):
             raise NotImplementedError(
-                "the fused sm_100a kernel is specialised for the reference defaults (model_args.py:10-19): "
+                "the fused sm_90a kernel is specialised for the reference defaults (model_args.py:10-19): "
                 "n_neurons=64, geometry_feature_dim=15, 1/2 hidden layers, sh_degree=4")
         if not 0 <= camera_embedding_dim <= 17:
             raise NotImplementedError("camera_embedding_dim must be in [0, 17] (16 SH + 15 geometry + E <= 48 inputs)")

@@ -68,8 +68,8 @@ class FusedTrainer:
         self.world, self.pg, self.prune, self.reuse = world_size, process_group, prune, reuse
         self.exchange = exchange if world_size > 1 else "local"
         # exchange="p2p", optional: run the exchange of hash grid k (barrier + reduce/Adam/shadow kernel on a side stream)
-        # while grid k+1 is still being scattered.  Measured on 2 B200s (profiles/r2_dp_2gpu_overlap_ab.txt): the exposed
-        # exchange shrinks 0.46 -> 0.39 ms but four per-grid scatter launches cost 0.15 ms more than one: off by default.
+        # while grid k+1 is still being scattered.  The exposed exchange shrinks, but four per-grid scatter launches cost
+        # more than one: off by default.
         self.overlap_exchange = bool(overlap_exchange) and self.exchange == "p2p"
         self.rank = dist.get_rank(process_group) if world_size > 1 else 0
         self.params: List[torch.nn.Parameter] = model.hot_parameters()
@@ -102,9 +102,8 @@ class FusedTrainer:
             sg[s_].vectors = self.grad_views[5 * s_ + 4].data_ptr()
         # HRF_VECGRAD_T=1 (experiment, off): the scatter accumulates the vector-row gradients in a transposed scratch
         # ([4][16][VR][2]: the rows neighbouring samples touch share 128-byte lines) and hrf_fold_vector_grads adds it into
-        # the bucket before Adam / the exchange read the gradient.  Measured on B200 (profiles/r2n_*): L2 RED requests
-        # 141 M -> 118 M, L1TEX 73 -> 57 %, L2 62 -> 50 % -- and the kernel SLOWER, 1.02 -> 1.09 ms: packing the adds of
-        # neighbouring lanes into the same lines makes them queue behind each other in the L2's atomic units.
+        # the bucket before Adam / the exchange read the gradient.  Fewer L2 RED requests, but not a faster kernel: packing
+        # the adds of neighbouring lanes into the same lines makes them queue behind each other in the L2's atomic units.
         self.vec_grad_t = None
         if os.environ.get("HRF_VECGRAD_T", "0") == "1":
             vn = self.grad_views[4].numel()
@@ -295,8 +294,8 @@ class FusedTrainer:
             head[0] = float(num_rays)
             if used is not None:
                 head[1:] = used.float()
-            # Asynchronous: the collective runs on NCCL's stream beside the prune pass (measured on 2 B200s: 0.11 ms per step
-            # when the prune pass waited for it); its result is first needed by the loss kernel.
+            # Asynchronous: the collective runs on NCCL's stream beside the prune pass instead of delaying it; its result is
+            # first needed by the loss kernel.
             head_work = dist.all_reduce(head, group=self.pg, async_op=True)
             launches += 6
         src = feat_src = None

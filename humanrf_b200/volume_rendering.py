@@ -1,4 +1,4 @@
-"""Volume renderer on the fused sm_100a kernels.
+"""Volume renderer on the fused sm_90a kernels.
 
 Drop-in for humanrf/volume_rendering.py:14-150: ``RenderOutput``, ``prune_samples`` (in-place,
 returns None) and ``render`` with the reference signatures.  Differences by design:

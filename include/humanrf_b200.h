@@ -1,5 +1,5 @@
 /*
- * humanrf_b200 -- C ABI of the B200-native (sm_100a) HumanRF per-ray hot path.
+ * humanrf_b200 -- C ABI of the H100-native (sm_90a) HumanRF per-ray hot path.
  *
  * Drop-in boundary for the reference's three pybind11 torch extensions and the two
  * third-party CUDA packages its hot path calls (SURVEY.md section 8b).  Every entry point
@@ -154,7 +154,7 @@ typedef struct {
 } hrf_samples;
 
 /* mode: 0 = density only (sigma, geo), 1 = density + radiance.  Any output may be NULL.
- * mlp_impl: 0 = tcgen05 tensor-core path (the product); 1 = SIMT fp32 debug path used only by
+ * mlp_impl: 0 = wgmma tensor-core path (the product); 1 = SIMT fp32 debug path used only by
  * tests to localise tensor-core descriptor faults. */
 int hrf_field_forward(const hrf_field* f, const hrf_samples* s, int mode, int mlp_impl,
                       float* sigma /* [N] */, void* geo_bf16 /* [N,16] (col 0 = raw h0) */,
@@ -231,10 +231,10 @@ typedef struct {
   float* grid[4];                    /* [n_entries,2] fp32, same order as hrf_segment.grid */
   float* vectors;                    /* [4, vec_res, 32] fp32 */
   /* Optional scratch in the transposed layout of hrf_segment.vectors_t, [4 axes][16 levels][vec_res][2], zeroed by the
-   * caller once.  When non-NULL the default scatter generation accumulates the vector-row gradient THERE instead of in
+   * caller once.  When non-NULL scatter generation 3 (scatter_v3.cu) accumulates the vector-row gradient THERE instead of in
    * `vectors`: the two tap rows of a sample, and the rows of the neighbouring samples of a ray, then share 128-byte lines
-   * (16 rows of one level per line instead of one row of 16 levels): 16 % fewer L2 RED requests per launch, but measured
-   * 6 % SLOWER on B200 (same-line adds queue in the L2 atomic units), so humanrf_b200.training leaves it NULL by default.
+   * (16 rows of one level per line instead of one row of 16 levels): fewer L2 RED requests per launch, but same-line adds
+   * queue in the L2 atomic units, and it was not faster; humanrf_b200.training leaves it NULL by default.
    * The caller folds it back with hrf_fold_vector_grads before anything reads `vectors`.  The other scatter
    * generations ignore the field and add into `vectors` directly, so the fold is always correct. */
   float* vectors_t;
@@ -306,7 +306,7 @@ int hrf_fold_vector_grads(float* vectors_t_grad, float* vectors_grad, int vec_re
  * counters live on the device (int32 per tensor, incremented here), so a step needs no host decision.  After reading
  * a gradient element the kernel writes 0 back when zero_grad != 0 (the bucket is then clean for the next backward).
  * blob_perm: for the MLP tensors, element i of the tensor is also written as bf16 to shadow[blob_perm[i]] (the packed
- * tcgen05 weight blob) instead of shadow[i]. */
+ * wgmma weight blob) instead of shadow[i]. */
 typedef struct {
   float* param; float* exp_avg; float* exp_avg_sq; float* grad;
   void* shadow_bf16;                 /* or NULL */
@@ -381,11 +381,11 @@ int hrf_occupancy_union_count(void* cluster_bits /* ceil(n/32) u32, caller-zeroe
                               int64_t num_voxels, int64_t* count_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Self tests (used by tests/ only): one 128xN x K tcgen05 MMA with caller-chosen descriptor
+ * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
 int hrf_selftest_umma(const void* a_bf16 /* [M,K] row-major */, const void* b_bf16 /* [N,K] row-major */,
-                      float* d /* [M,N] */, int m /* 64 or 128 */, int n, int k,
+                      float* d /* [M,N] */, int m /* 64 or 128 */, int n /* 16, 32, 48 or 64 */, int k,
                       /* physical placement of the 8x8 core matrices in shared memory (bytes) */
                       uint32_t a_kstride, uint32_t a_mstride, uint32_t b_kstride, uint32_t b_nstride,
                       /* descriptor fields (bytes) */

@@ -25,7 +25,7 @@ PARITY PINNING STATUS (see DESIGN.md "Oracle"):
   * first-party CUDA (``tensor_composition.cu``, ``ray_sampler.cu``, ``occupancy_grid.cu``,
     ``occupancy_grid_generation.cu``) is pinned on the GPU box against ``oracle/_ref`` builds
     of the reference sources (``oracle/build_ref.py``) when those built here.
-  * tiny-cuda-nn (un-pinned git HEAD) and nerfacc==0.3.1 are NOT under /root/reference and
+  * tiny-cuda-nn (un-pinned git HEAD) and nerfacc==0.3.1 are NOT part of the reference checkout and
     cannot be installed here: their published algorithms are restated from memory of the
     public sources and are **parity unpinned**.
 """

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY.  Compiles the reference's own first-party CUDA extensions from the
-sources where they lie under /root/reference (nothing is copied) into oracle/_ref/ so the GPU
-box can diff our kernels against the real thing:
+sources where they lie in a checkout of the reference (nothing is copied) into oracle/_ref/, so that
+tests/golden/make_ref_parity_golden.py can record what the real thing computes:
 
   tensor_composition_native  <- humanrf/scene_representation/native/tensor_composition.cu
   occupancy_grid_native      <- actorshq/dataset/native/occupancy_grid.cu
@@ -8,8 +8,9 @@ box can diff our kernels against the real thing:
   occupancy_grid_generation_native <- actorshq/toolbox/native/occupancy_grid_generation.cu   (+ oracle/glm_shim)
 
 Flags follow humanrf/setup.py:17 and actorshq/setup.py:17-29 (--use_fast_math) with the arch
-pinned to sm_100.  tinycudann / nerfacc are not under /root/reference and cannot be built.
-Run:  python oracle/build_ref.py   (a few minutes per extension; skipped when up to date)
+pinned to sm_90.  tinycudann / nerfacc are not part of the reference checkout and cannot be built.
+Run:  HUMANRF_REFERENCE=<path to the reference checkout> python oracle/build_ref.py
+(a few minutes per extension; skipped when up to date)
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ import sys
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
-REF = Path("/root/reference")
+REF = Path(os.environ.get("HUMANRF_REFERENCE", ""))
 OUT = HERE / "_ref"
 
 EXTS = {
@@ -31,10 +32,10 @@ EXTS = {
 
 
 def build(names=None, verbose=False):
-    if not REF.exists():
-        print("reference sources not present; skipping oracle/_ref build")
+    if not os.environ.get("HUMANRF_REFERENCE") or not REF.exists():
+        print("HUMANRF_REFERENCE does not name a reference checkout; skipping oracle/_ref build")
         return {}
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0"
     from torch.utils.cpp_extension import load  # noqa: WPS433
 
     OUT.mkdir(exist_ok=True)

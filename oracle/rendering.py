@@ -5,7 +5,7 @@ humanrf/trainer.py:205-255, humanrf/utils/loss.py:4-10.  The first-party glue (p
 jitter, alpha, t_ends = t + step, mask application, background blend) is PINNED: the
 reference's own prune_samples / render run on the CPU and agree bit for bit
 (tests/test_reference_live_cpu.py).  PARITY UNPINNED for the nerfacc==0.3.1 pieces
-(requirements.txt:3, not under /root/reference): restated from its published semantics
+(requirements.txt:3, not part of the reference checkout): restated from its published semantics
 (nerfacc/vol_rendering.py: render_visibility, render_weight_from_density,
 accumulate_along_rays).
 """

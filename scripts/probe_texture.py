@@ -1,5 +1,5 @@
 """GPU experiment (test infrastructure): dump raw hardware tex3D values for controlled sub-texel offsets so the
-1.8 fixed-point emulation can be fitted exactly.  Writes gpurun_out/texprobe.npz."""
+1.8 fixed-point emulation can be fitted exactly.  usage: python scripts/probe_texture.py <output .npz>"""
 import ctypes
 import sys
 from pathlib import Path
@@ -65,5 +65,5 @@ rng = np.random.default_rng(1)
 r = rng.uniform(-1.2, 2.2, (300000, 3))
 pts = ((32 + 0.5 + r) / G).astype(np.float32)
 out["F_p"], out["F_v"] = pts, hw(grid, pts)
-np.savez_compressed(ROOT / "gpurun_out/texprobe.npz", **out)
-print("wrote texprobe.npz")
+np.savez_compressed(sys.argv[1], **out)
+print("wrote", sys.argv[1])

@@ -1,4 +1,4 @@
-"""Gradient parity of the fused backward kernel (MLP dgrad/wgrad on tcgen05, table/vector scatter)
+"""Gradient parity of the fused backward kernel (MLP dgrad/wgrad on wgmma, table/vector scatter)
 with torch autograd through the CPU oracle.  Gradient tiles are bf16 inside the kernel, so the bar is
 norm-wise: |g - g_ref| / |g_ref| <= 3e-2 per parameter tensor (and the touched-entry pattern matches)."""
 import numpy as np

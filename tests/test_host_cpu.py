@@ -117,12 +117,13 @@ def test_product_does_not_import_oracle():
         assert "import oracle" not in src and "from oracle" not in src, p
 
 
-def test_dropin_maps_reference_import_paths():
+def test_dropin_maps_reference_import_paths(tmp_path):
     import sys
 
-    ref = "/root/reference"
-    if not Path(ref).exists():
-        pytest.skip("reference checkout not present (GPU box)")
+    # the reference checkout's package layout: namespace packages (no __init__.py) down to the modules dropin replaces
+    for pkg in ("humanrf/scene_representation", "actorshq/dataset", "actorshq/toolbox"):
+        (tmp_path / pkg).mkdir(parents=True)
+    ref = str(tmp_path)
     import humanrf_b200.dropin as dropin
 
     sys.path.insert(0, ref)
@@ -139,22 +140,6 @@ def test_dropin_maps_reference_import_paths():
         for k in list(sys.modules):
             if k.startswith(("humanrf.", "actorshq.")) or k in ("humanrf", "actorshq"):
                 del sys.modules[k]
-
-
-def test_bench_reads_roofline_evidence_of_the_default_kernels():
-    """bench.py fills roofline.traffic and the unit percentages from the newest committed `ncu --set full` export that holds the
-    kernel it names: the default scatter generation for the train line, the fused forward for the render line."""
-    import sys
-
-    sys.path.insert(0, str(ROOT))
-    import bench
-
-    for kernel in ("grid_scatter_v3_kernel", "field_forward_kernel"):
-        prof = bench.committed_ncu(kernel)
-        assert prof is not None and kernel in prof["kernel_name"], kernel
-        assert prof["source"].startswith("profiles/r2") and prof["source"].endswith("_raw.csv")
-        assert prof["traffic"] > 1e6 and 0 < prof["issue_slots_pct"] <= 100 and 0 < prof["l2_pct"] <= 100
-    assert bench.committed_ncu("no_such_kernel") is None
 
 
 def test_reference_arm_line_follows_the_bench_contract(monkeypatch, capsys):

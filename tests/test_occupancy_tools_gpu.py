@@ -1,9 +1,6 @@
-"""SURVEY 8f-4 on the GPU: visual-hull carving bit-exact against the oracle and statistically against the reference's
-own extension (oracle/_ref); adaptive temporal partitioning against the reference's golden decisions."""
-import importlib
-import sys
-from pathlib import Path
-
+"""SURVEY 8f-4 on the GPU: visual-hull carving bit-exact against the oracle and statistically against what the reference's
+own extension computes (stored in tests/golden/ref_parity.npz, see test_ref_parity_gpu.py); adaptive temporal partitioning
+against the reference's golden decisions."""
 import numpy as np
 import pytest
 import torch
@@ -13,7 +10,6 @@ from scene import carve_scene, occupancy_sequence
 from test_occupancy_tools_cpu import golden_cases
 
 pytestmark = pytest.mark.gpu
-REF = Path(__file__).resolve().parent.parent / "oracle" / "_ref"
 
 
 def _carve(sc, thr, G, cuda):
@@ -39,36 +35,41 @@ def test_carve_rejects_wrong_mask_size(cuda):
         _carve(dict(sc, width=31), 1, 8, cuda)
 
 
+CARVE_G, CARVE_THR = 256, 20
+
+
+def _carve_args(cuda):
+    sc = carve_scene(num_cameras=24, width=512, height=384, seed=5)
+    return (torch.from_numpy(sc["masks"]).to(cuda), torch.from_numpy(sc["projection_matrices"]).to(cuda),
+            torch.from_numpy(sc["landscape"]).to(cuda), CARVE_THR, CARVE_G, 512, 384)
+
+
+def reference_carve(ref, cuda):
+    want = ref("occupancy_grid_generation_native").generate_from_masks(*_carve_args(cuda)).cpu().numpy()
+    assert set(np.unique(want).tolist()) <= {0, 255}
+    return {"carve/occupied_bits": np.packbits(want.reshape(-1) == 255)}
+
+
 def test_carve_vs_reference_extension(cuda):
     """Full-size carve (G=256, 24 cameras) against the reference's kernel built from its unmodified source.  The
     reference is compiled with --use_fast_math (approximate divides), so a voxel whose projection lands within an ulp
     of a pixel boundary may sample a neighbouring mask pixel: a handful of voxels out of 16.7 M."""
-    if not (REF / "occupancy_grid_generation_native.so").exists():
-        pytest.skip("oracle/_ref/occupancy_grid_generation_native.so not built")
-    if str(REF) not in sys.path:
-        sys.path.insert(0, str(REF))
-    ref = importlib.import_module("occupancy_grid_generation_native")
-    sc = carve_scene(num_cameras=24, width=512, height=384, seed=5)
-    G, thr = 256, 20
-    args = (torch.from_numpy(sc["masks"]).to(cuda), torch.from_numpy(sc["projection_matrices"]).to(cuda),
-            torch.from_numpy(sc["landscape"]).to(cuda), thr, G, 512, 384)
-    want = ref.generate_from_masks(*args)
     from humanrf_b200.toolbox import occupancy_grid_generation_native as ours
+    from test_ref_parity_gpu import GOLD
 
+    G = CARVE_G
+    want = np.unpackbits(np.load(GOLD)["carve/occupied_bits"])[:G ** 3].astype(np.uint8) * 255
+    args = _carve_args(cuda)
     got = ours.generate_from_masks(*args)
     torch.cuda.synchronize()
-    diff = int((want != got).sum())
+    diff = int((want != got.cpu().numpy().reshape(-1)).sum())
     occ = int((want == 255).sum())
-    def ms(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        fn(); e0.record()
-        for _ in range(5):
-            fn()
-        e1.record(); torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / 5
-
-    print(f"carve vs reference: {diff} of {G ** 3} voxels differ, {occ} occupied; "
-          f"ours {ms(lambda: ours.generate_from_masks(*args)):.3f} ms, reference {ms(lambda: ref.generate_from_masks(*args)):.3f} ms")
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(5):
+        ours.generate_from_masks(*args)
+    e1.record(); torch.cuda.synchronize()
+    print(f"carve vs reference: {diff} of {G ** 3} voxels differ, {occ} occupied; ours {e0.elapsed_time(e1) / 5:.3f} ms")
     assert 0 < occ < G ** 3 and diff <= 2e-5 * G ** 3
 
 

@@ -1,4 +1,4 @@
-"""Bit-exact parity of the sm_100a sampler (csrc/sampler.cu) with oracle/sampler.py, which restates
+"""Bit-exact parity of the sm_90a sampler (csrc/sampler.cu) with oracle/sampler.py, which restates
 ray_sampler.cu:11-194,196-325 in canonical IEEE float32 arithmetic, for all four entry points, a
 CPU- and a GPU-resident image pool, landscape/portrait images, light-bloom filtering."""
 import numpy as np

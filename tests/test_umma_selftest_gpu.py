@@ -1,4 +1,4 @@
-"""Pins the tcgen05 shared-memory descriptor encoding on real hardware: one 128xNxK (and 64xNxK,
+"""Pins the wgmma shared-memory descriptor encoding on real hardware: one 128xNxK (and 64xNxK,
 and MN-major) MMA through hrf_selftest_umma against torch.  If the expected (LBO,SBO) reading is
 wrong, the failing assert prints which alternative matches."""
 import pytest
