@@ -110,6 +110,8 @@ _SIGNATURES = {
     "hrf_fold_vector_grads": (C.c_int, [vp, vp, C.c_int, vp]),
     "hrf_occupancy_from_masks": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "hrf_occupancy_union_count": (C.c_int, [vp, vp, i64, vp, vp]),
+    "hrf_bake_occupancy_workspace_bytes": (i64, [C.c_int]),
+    "hrf_bake_occupancy": (C.c_int, [C.POINTER(Field), i32, vp, C.c_int, f32, f32, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

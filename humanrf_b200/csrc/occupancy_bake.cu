@@ -1,0 +1,192 @@
+// Learned occupancy grid for inference: the trained density field evaluated over the occupied voxels of a hull grid
+// (include/humanrf_b200.h, hrf_bake_occupancy).  Three launches, no host read:
+//   hull_compact_kernel : ids of the hull's occupied voxels -> device list + device count; zeroes `live` / max_sigma
+//                         outside the hull
+//   occupancy_bake_kernel: persistent, one warpgroup per CTA, 128-row tiles of 16 voxels x 8 sub-samples: positions
+//                         generated in the kernel -> encode -> sigma MLP (wgmma) -> density -> per-voxel max (3 xor
+//                         shuffles over the voxel's 8 consecutive lanes) -> max_sigma, live byte
+//   dilate_and_kernel   : out = hull AND (26-neighbourhood dilation of live by one voxel), {0,255}
+// The density of a sub-sample is bit for bit what hrf_field_forward (mode 0, query form) returns for its position: the
+// same encode_to_smem, the same two wgmma layers and the same epilogue.
+#include "field_mlp.cuh"
+
+namespace hrf {
+
+constexpr int kBakeVoxelsPerTile = kTile / 8;   // 16 voxels x 8 sub-samples = one 128-row tile
+constexpr int kBakeCtasPerSm = 5;
+constexpr int64_t kBakeHeaderBytes = 256;       // device count, then the id list
+
+__global__ void __launch_bounds__(256) hull_compact_kernel(const uint8_t* __restrict__ hull, uint32_t n,
+                                                           int32_t* __restrict__ count, int32_t* __restrict__ ids,
+                                                           uint8_t* __restrict__ live, float* __restrict__ max_sigma) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool in = v < n;
+  const bool occ = in && hull[v] != 0;
+  const uint32_t b = __ballot_sync(0xffffffffu, occ);
+  const int lane = threadIdx.x & 31;
+  int base = 0;
+  if (lane == 0 && b != 0u) base = atomicAdd(count, __popc(b));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (occ) {
+    ids[base + __popc(b & ((1u << lane) - 1u))] = (int32_t)v;
+  } else if (in) {   // hull voxels are written by the bake kernel
+    live[v] = 0;
+    if (max_sigma != nullptr) max_sigma[v] = 0.f;
+  }
+}
+
+struct BakeArgs {
+  hrf_field f;
+  const int32_t* count;
+  const int32_t* ids;
+  int32_t frame, G;
+  float step, alpha_thre;
+  uint8_t* live;
+  float* max_sigma;
+};
+
+// Sub-sample position along one axis: the cell-centred convention of the texture lookup the sampler emulates (voxel i
+// covers [i/G, (i+1)/G) of p + 0.5), sub-samples at 1/4 and 3/4 of the cell.
+__device__ __forceinline__ float bake_coord(int i, int half, float G) {
+  return __fsub_rn(__fdiv_rn((float)i + 0.25f + 0.5f * (float)half, G), 0.5f);
+}
+
+__global__ void __launch_bounds__(kTile, kBakeCtasPerSm) occupancy_bake_kernel(const __grid_constant__ BakeArgs args) {
+  extern __shared__ unsigned char smem_raw[];
+  FwdSmem& sm = *reinterpret_cast<FwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  const int tid = threadIdx.x;
+  const hrf_field& f = args.f;
+
+  // only the sigma net is evaluated: its two layers are the first kWCol1 bytes of the blob, whatever the colour net's width
+  if (tid == 0) {
+    mbar_init(&sm.bar_w, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&sm.bar_w, kWCol1);
+    tma_load_1d(sm.w, f.mlp_blob, kWCol1, &sm.bar_w);
+  }
+  bool weights_ready = false;
+
+  // frame -> segment and normalised local time, once (the host checked that the frame lies inside the LUT)
+  const int sg = __ldg(f.frame_to_segment + args.frame);
+  const float t_local = __ldg(f.frame_to_tlocal + args.frame);
+  const hrf_segment* seg = (sg >= 0 && sg < f.num_segments) ? f.segments + sg : nullptr;
+
+  const int64_t nvox = *reinterpret_cast<const volatile int32_t*>(args.count);
+  const int64_t num_tiles = (nvox + kBakeVoxelsPerTile - 1) / kBakeVoxelsPerTile;
+  const int G = args.G;
+  const float Gf = (float)G;
+  const int slot = tid >> 3, sub = tid & 7;
+  for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int64_t k = tile * kBakeVoxelsPerTile + slot;
+    const bool valid = k < nvox;
+    const int32_t vid = valid ? __ldg(args.ids + k) : 0;
+    Sample s;
+    s.seg = valid ? seg : nullptr;
+    s.t = t_local;
+    {
+      const int x = vid % G, yz = vid / G, y = yz % G, z = yz / G;
+      // humanrf.py:175 (positions + 0.5), as load_sample does for a query-form position
+      s.x = __fadd_rn(bake_coord(x, sub & 1, Gf), 0.5f);
+      s.y = __fadd_rn(bake_coord(y, (sub >> 1) & 1, Gf), 0.5f);
+      s.z = __fadd_rn(bake_coord(z, sub >> 2, Gf), 0.5f);
+    }
+    encode_to_smem<false, 1>(f, s, sm.a, tid);
+    if (!weights_ready) {
+      mbar_wait(&sm.bar_w, 0);
+      weights_ready = true;
+    }
+    run_hidden<false, 32>(sm, kWSig1);
+    float o[16];
+    run_layer16<false, 64>(sm, kWSig2, o);
+    // humanrf.py:184 : density = truncated_exp(h[...,0]) * density_scale, exactly the forward's epilogue
+    float m = __expf(o[0]) * f.density_scale;
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+    if (valid && sub == 0) {
+      if (seg == nullptr) m = 0.f;
+      if (args.max_sigma != nullptr) args.max_sigma[vid] = m;
+      // composite.cu visibility_kernel: alpha = 1 - exp(-sigma * step), kept when alpha >= alpha_thre
+      args.live[vid] = (1.f - expf(-m * args.step) >= args.alpha_thre) ? 1 : 0;
+    }
+  }
+  if (!weights_ready) mbar_wait(&sm.bar_w, 0);  // never leave a bulk copy in flight
+}
+
+// out = hull AND (any live voxel in the 3x3x3 neighbourhood), one thread per voxel; `live` is 0 outside the hull.
+__global__ void __launch_bounds__(256) dilate_and_kernel(const uint8_t* __restrict__ hull, const uint8_t* __restrict__ live,
+                                                         int G, uint8_t* __restrict__ out) {
+  const uint32_t n = (uint32_t)G * (uint32_t)G * (uint32_t)G;
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n) return;
+  bool any = false;
+  if (hull[v] != 0) {
+    const int x = (int)(v % (uint32_t)G), yz = (int)(v / (uint32_t)G), y = yz % G, z = yz / G;
+    for (int dz = -1; dz <= 1 && !any; ++dz) {
+      const int zz = z + dz;
+      if (zz < 0 || zz >= G) continue;
+      for (int dy = -1; dy <= 1 && !any; ++dy) {
+        const int yy = y + dy;
+        if (yy < 0 || yy >= G) continue;
+        const uint8_t* row = live + ((uint32_t)zz * (uint32_t)G + (uint32_t)yy) * (uint32_t)G;
+        for (int dx = -1; dx <= 1; ++dx) {
+          const int xx = x + dx;
+          if (xx >= 0 && xx < G && __ldg(row + xx) != 0) any = true;
+        }
+      }
+    }
+  }
+  out[v] = any ? 255 : 0;
+}
+
+}  // namespace hrf
+
+using namespace hrf;
+
+extern "C" int64_t hrf_bake_occupancy_workspace_bytes(int grid_resolution) {
+  if (grid_resolution < 1 || grid_resolution > 1024) return 0;
+  const int64_t n = (int64_t)grid_resolution * grid_resolution * grid_resolution;
+  return kBakeHeaderBytes + ((4 * n + 255) / 256) * 256 + n;
+}
+
+extern "C" int hrf_bake_occupancy(const hrf_field* f, int32_t frame_number, const uint8_t* hull_u8, int grid_resolution,
+                                  float step, float alpha_thre, uint8_t* out_u8, float* max_sigma, void* workspace,
+                                  void* stream) {
+  HRF_REQUIRE(f != nullptr && hull_u8 != nullptr && out_u8 != nullptr && workspace != nullptr, "null argument");
+  HRF_REQUIRE(f->mlp_blob != nullptr && f->segments != nullptr && f->frame_to_segment != nullptr, "field not initialised");
+  HRF_REQUIRE(grid_resolution >= 1 && grid_resolution <= 1024, "grid resolution must be in [1, 1024] (int32 voxel ids)");
+  HRF_REQUIRE(frame_number >= 0 && frame_number < f->lut_size, "frame number outside the model's frame table");
+  HRF_REQUIRE(step > 0.f && alpha_thre > 0.f && alpha_thre < 1.f, "step must be positive and alpha_thre in (0, 1)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int64_t n = (int64_t)grid_resolution * grid_resolution * grid_resolution;
+  char* ws = reinterpret_cast<char*>(workspace);
+  int32_t* count = reinterpret_cast<int32_t*>(ws);
+  int32_t* ids = reinterpret_cast<int32_t*>(ws + kBakeHeaderBytes);
+  uint8_t* live = reinterpret_cast<uint8_t*>(ws + kBakeHeaderBytes + ((4 * n + 255) / 256) * 256);
+  HRF_CUDA(cudaMemsetAsync(count, 0, sizeof(int32_t), st));
+  const unsigned blocks = (unsigned)((n + 255) / 256);
+  hull_compact_kernel<<<blocks, 256, 0, st>>>(hull_u8, (uint32_t)n, count, ids, live, max_sigma);
+  HRF_CHECK_LAUNCH();
+
+  BakeArgs a;
+  a.f = *f;
+  a.count = count, a.ids = ids;
+  a.frame = frame_number, a.G = grid_resolution;
+  a.step = step, a.alpha_thre = alpha_thre;
+  a.live = live, a.max_sigma = max_sigma;
+  const int smem = (int)(offsetof(FwdSmem, w) + kWCol1) + 128;
+  // persistent: the voxel count stays on the device, so the grid is sized to one full wave and every CTA walks tiles
+  const int64_t max_tiles = (n + kBakeVoxelsPerTile - 1) / kBakeVoxelsPerTile;
+  const int64_t wave = (int64_t)sm_count() * kBakeCtasPerSm;
+  const int grid = (int)(max_tiles < wave ? max_tiles : wave);
+  HRF_CUDA(cudaFuncSetAttribute(occupancy_bake_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  occupancy_bake_kernel<<<grid, kTile, smem, st>>>(a);
+  HRF_CHECK_LAUNCH();
+
+  dilate_and_kernel<<<blocks, 256, 0, st>>>(hull_u8, live, grid_resolution, out_u8);
+  HRF_CHECK_LAUNCH();
+  return 0;
+}

@@ -80,6 +80,7 @@ class HumanRF(torch.nn.Module):
             raise NotImplementedError("camera_embedding_dim must be in [0, 17] (16 SH + 15 geometry + E <= 48 inputs)")
         self.density_scale = float(density_scale)
         self.num_frames = len(sorted_frame_numbers)
+        self.sorted_frame_numbers = tuple(int(f) for f in sorted_frame_numbers)
         self.num_segments = len(segment_sizes)
         self.camera_embedding_dim = camera_embedding_dim
         if camera_embedding_dim > 0:

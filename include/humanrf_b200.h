@@ -381,6 +381,29 @@ int hrf_occupancy_union_count(void* cluster_bits /* ceil(n/32) u32, caller-zeroe
                               int64_t num_voxels, int64_t* count_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Learned occupancy grid for inference: the trained density field evaluated over the occupied voxels of a hull grid
+ * (uint8 [G][G][G] indexed [z][y][x], non-zero = occupied, 255 as hrf_occupancy_from_masks writes it).  The result is a
+ * tighter grid in the format hrf_occgrid_add takes.  For every hull voxel (x, y, z):
+ *   1. eight sub-sample positions, a, b, c in {0,1}:
+ *        px = __fsub_rn(__fdiv_rn((float)x + 0.25f + 0.5f*a, (float)G), 0.5f), and the same for py (b) and pz (c)
+ *      (the texture lookup's cell-centred convention: voxel i covers [i/G, (i+1)/G) of p + 0.5);
+ *   2. sigma = exactly what hrf_field_forward (mode 0, query form) returns for that position and frame; m = max of the 8;
+ *   3. live = (1.f - expf(-m * step) >= alpha_thre), the alpha test of hrf_prune: a voxel is dead only if pruning would
+ *      drop every one of its sub-samples;
+ *   4. out = hull AND dilate(live), a one-voxel 26-neighbourhood dilation that never leaves the hull, values {0,255};
+ *   5. max_sigma (optional, float32 [G^3]) = m on hull voxels, 0 elsewhere.
+ * Meant for rendering (step = render_step_size 4e-4, alpha_thre = 1e-4 as hrf_prune is called); training keeps its
+ * hull grids.  Reads the sigma part of the MLP blob only, so models with camera embeddings are handled.  The hull's
+ * voxel count stays on the device: nothing here synchronises.  G must be in [1, 1024] and the frame inside the
+ * model's frame table; a frame of the table that belongs to no segment gives an all-zero grid (the Python entry
+ * point rejects it).  workspace: hrf_bake_occupancy_workspace_bytes(G) bytes of device scratch.
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_bake_occupancy_workspace_bytes(int grid_resolution);
+int hrf_bake_occupancy(const hrf_field* f, int32_t frame_number, const uint8_t* hull_u8 /* [G^3] */, int grid_resolution,
+                       float step, float alpha_thre, uint8_t* out_u8 /* [G^3] */, float* max_sigma /* [G^3] or NULL */,
+                       void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
