@@ -112,6 +112,11 @@ _SIGNATURES = {
     "hrf_occupancy_union_count": (C.c_int, [vp, vp, i64, vp, vp]),
     "hrf_bake_occupancy_workspace_bytes": (i64, [C.c_int]),
     "hrf_bake_occupancy": (C.c_int, [C.POINTER(Field), i32, vp, C.c_int, f32, f32, vp, vp, vp, vp]),
+    "hrf_density_lattice_workspace_bytes": (i64, [C.c_int]),
+    "hrf_density_lattice": (C.c_int, [C.POINTER(Field), i32, vp, C.c_int, vp, vp, vp]),
+    "hrf_marching_cubes_workspace_bytes": (i64, [C.c_int]),
+    "hrf_marching_cubes_count": (C.c_int, [vp, C.c_int, f32, vp, vp, vp]),
+    "hrf_marching_cubes_emit": (C.c_int, [vp, C.c_int, f32, i64, i64, vp, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

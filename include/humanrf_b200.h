@@ -404,6 +404,49 @@ int hrf_bake_occupancy(const hrf_field* f, int32_t frame_number, const uint8_t* 
                        void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Mesh extraction: a density lattice at the corners of a G^3 grid's voxels, then marching cubes over it.
+ *
+ * hrf_density_lattice: sigma [(G+1)^3] fp32 indexed [k][j][i] (z, y, x).  Vertex (i, j, k), i, j, k in [0, G], sits at
+ *   p = __fsub_rn(__fdiv_rn((float)i, (float)G), 0.5f) per axis: the corners of the voxels of hrf_bake_occupancy's
+ *   cell-centred convention, so the cubes of marching cubes are exactly the grid's voxels.  sigma at a vertex that is a
+ *   corner of at least one occupied mask voxel (uint8 [G^3], non-zero = occupied; mask NULL = every vertex) is exactly
+ *   what hrf_field_forward (mode 0, query form) returns at that position and frame; every other vertex gets 0.  The
+ *   vertex count stays on the device: nothing here synchronises.  G in [1, 1024], the frame inside the model's frame
+ *   table.  workspace: hrf_density_lattice_workspace_bytes(G) bytes of device scratch.
+ *
+ * hrf_marching_cubes_count / _emit: the surface {sigma >= level} of any fp32 lattice [(G+1)^3] indexed [k][j][i].
+ *   - inside <=> sigma >= level; a lattice edge crosses <=> exactly one endpoint is inside.
+ *   - one mesh vertex per crossing lattice edge, owned by its lower endpoint; vertices are numbered in the order
+ *     (owner's linear index i + (G+1)(j + (G+1)k), axis x < y < z).  With s0 at the lower endpoint,
+ *     t = __fdiv_rn(__fsub_rn(level, s0), __fsub_rn(s1, s0)); the coordinate along the edge's axis is
+ *     __fsub_rn(__fdiv_rn(__fadd_rn((float)i, t), (float)G), 0.5f), the other two are the owner's lattice coordinates.
+ *     Neighbouring cubes share vertex ids: the mesh is indexed.
+ *   - faces (int32 [F,3]) in the order of the cube's linear index, then of the case table; they wind counter-clockwise
+ *     seen from the outside (lower sigma): the geometric normal points toward decreasing sigma.
+ *   - case table, generated from a face rule: on a cube face with two crossing edges they are joined; with four, the
+ *     two edges at each inside corner are joined (inside corners are not connected across a face).  The segments chain
+ *     into loops, taken from the smallest unused crossing edge (cube edge e = 4 axis + idx, idx = the other two corner
+ *     bits in axis order) and fan-triangulated from their first vertex whose diagonals join no two edges of a common
+ *     cube face.  Both cubes sharing a face draw the same segments there, so the mesh is closed wherever the lattice
+ *     border is outside.
+ *   - normals (optional, fp32 [V,3]): -grad sigma from central differences on the lattice (one-sided at its border),
+ *     interpolated along the edge by t, then normalised (0 where the gradient vanishes).
+ *   Deterministic: places come from prefix sums, two runs write identical bytes.
+ *   _count writes counts[2] = {V, F} (device int64).  The caller reads them back -- the only host synchronisation of an
+ *   extraction -- sizes the outputs and calls _emit with the same lattice, level and workspace.  V must fit int32.
+ *   workspace: hrf_marching_cubes_workspace_bytes(G) bytes, kept between the two calls.
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_density_lattice_workspace_bytes(int grid_resolution);
+int hrf_density_lattice(const hrf_field* f, int32_t frame_number, const uint8_t* mask_u8 /* [G^3] or NULL */,
+                        int grid_resolution, float* sigma /* [(G+1)^3] */, void* workspace, void* stream);
+int64_t hrf_marching_cubes_workspace_bytes(int grid_resolution);
+int hrf_marching_cubes_count(const float* lattice /* [(G+1)^3] */, int grid_resolution, float level,
+                             int64_t* counts /* [2] device */, void* workspace, void* stream);
+int hrf_marching_cubes_emit(const float* lattice, int grid_resolution, float level, int64_t num_vertices,
+                            int64_t num_faces, float* vertices /* [V,3] */, float* normals /* [V,3] or NULL */,
+                            int32_t* faces /* [F,3] */, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
