@@ -85,6 +85,7 @@ _SIGNATURES = {
     "hrf_field_forward_from_features": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, vp, vp]),
     "hrf_render_fused_workspace_bytes": (i64, [i64]),
     "hrf_render_fused": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, i64, f32, vp, vp, vp, vp, vp, vp, vp]),
+    "hrf_render_fused_depth": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, i64, f32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "hrf_density_early_stop_workspace_bytes": (i64, [i64]),
     "hrf_field_density_early_stop": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, i64, f32, f32, vp, vp, vp, vp, vp]),
     "hrf_ray_offsets": (C.c_int, [vp, i64, i64, vp, vp]),

@@ -47,7 +47,8 @@ struct Composite {
   const float* background;      // [R,3] or NULL
   float* color;                 // [R,3]
   float* wsum;                  // [R]
-  float* partial;               // [tiles][2][8]: (optical depth, C.r, C.g, C.b, W) of the ray segments cut by a tile border
+  float* partial;               // [tiles][2][8]: (optical depth, C.r, C.g, C.b, W, [depth variant] sum w*t_mid) of the
+                                // ray segments cut by a tile border
   float step;
 };
 
@@ -64,6 +65,9 @@ struct FieldArgs {
   const uint4* feat_in;       // bf16 [M,32] composed features of an earlier pass (kFromFeat kernels: no encode)
   const int32_t* feat_index;  // row of feat_in per sample, or NULL (identity)
   int mode;
+  // [R] sum of w * t_mid per ray (kDepth compositing kernels only).  Kept last and out of Composite: the offsets of the
+  // members above are the kernel-parameter offsets every other field kernel was compiled against.
+  float* depth;
 };
 
 // Live number of samples: the device scalar of a sync-free pipeline (bounded by the capacity), or the host value.

@@ -27,8 +27,13 @@ __device__ __forceinline__ float warp_sum_fwd(float v) {
 // last: whole rays are finished here; the (at most two) cut segments leave a 5-float partial
 // (optical depth, transmittance-weighted colour and weight relative to the segment start) that composite_fixup_kernel
 // chains in tile order.  Segmented warp-shuffle scans keyed by the ray index; warps are joined through 3 words of smem.
-template <bool kSimt, int kCtasPerSm, bool kSaveGrid = false, int kLevelUnroll = 4, bool kFromFeat = false, bool kComposite = false>
+// kDepth (kComposite only): one more scan, of w * t_mid with t_mid = (t + (t + step)) / 2, gives each ray the unnormalised
+// expected distance sum w * t_mid (args.depth; slot 5 of a cut segment's partial).  The other scans are unchanged, so
+// colour and weights sum are bit-identical to those of the kernel without it.
+template <bool kSimt, int kCtasPerSm, bool kSaveGrid = false, int kLevelUnroll = 4, bool kFromFeat = false, bool kComposite = false,
+          bool kDepth = false>
 __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const __grid_constant__ FieldArgs args) {
+  static_assert(kComposite || !kDepth, "the depth scan is part of the compositing epilogue");
   extern __shared__ unsigned char smem_raw[];
   FwdSmem& sm = *reinterpret_cast<FwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   const int tid = threadIdx.x;
@@ -153,15 +158,18 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
     }
     if constexpr (kComposite) {
       // The activation tile is free (the last MMA that read it has committed): its first bytes join the four warps.
+      constexpr int kTail = kDepth ? 6 : 5;                 // scanned quantities per warp
       int* x_first = reinterpret_cast<int*>(sm.a);          // [4] ray of lane 0
       int* x_last = x_first + 4;                            // [4] ray of lane 31
-      float* x_tail = reinterpret_cast<float*>(x_first + 8);  // [4][5] inclusive sums of the warp's last ray at lane 31
+      float* x_tail = reinterpret_cast<float*>(x_first + 8);  // [4][kTail] inclusive sums of the warp's last ray at lane 31
       const int lane = tid & 31, warp = tid >> 5;
       const int ray = valid ? (int)__ldg(args.s.ray_indices + i) : -1;
       float sdt = 0.f;
+      float tmid = 0.f;
       if (valid) {
         const float t = __ldg(args.s.sample_distances + i);
         sdt = sigma * __fsub_rn(__fadd_rn(t, args.comp.step), t);   // sigmas * (t_ends - t_starts), volume_rendering.py:124-129
+        if constexpr (kDepth) tmid = __fmul_rn(0.5f, __fadd_rn(t, __fadd_rn(t, args.comp.step)));   // (t_starts + t_ends) / 2
       }
       auto seg_scan = [&](float v) {   // inclusive sum over the lanes of this warp that carry the same ray
 #pragma unroll
@@ -176,7 +184,7 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
         float c = 0.f;
         for (int w = warp - 1; w >= 0; --w) {
           if (x_last[w] != ray) break;
-          c += x_tail[w * 5 + k];
+          c += x_tail[w * kTail + k];
           if (x_first[w] != ray) break;
         }
         return c;
@@ -184,14 +192,18 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
       float depth = seg_scan(sdt);
       __syncthreads();   // every thread is done with the tile's operands
       if (lane == 0) x_first[warp] = ray;
-      if (lane == 31) x_last[warp] = ray, x_tail[warp * 5] = depth;
+      if (lane == 31) x_last[warp] = ray, x_tail[warp * kTail] = depth;
       __syncthreads();
       depth += carry_in(0);
       const float wgt = valid ? __expf(-(depth - sdt)) * (1.f - __expf(-sdt)) : 0.f;
       float a0 = seg_scan(wgt * c0), a1 = seg_scan(wgt * c1), a2 = seg_scan(wgt * c2), a3 = seg_scan(wgt);
-      if (lane == 31) x_tail[warp * 5 + 1] = a0, x_tail[warp * 5 + 2] = a1, x_tail[warp * 5 + 3] = a2, x_tail[warp * 5 + 4] = a3;
+      float a4 = 0.f;
+      if constexpr (kDepth) a4 = seg_scan(wgt * tmid);
+      if (lane == 31) x_tail[warp * kTail + 1] = a0, x_tail[warp * kTail + 2] = a1, x_tail[warp * kTail + 3] = a2, x_tail[warp * kTail + 4] = a3;
+      if constexpr (kDepth) if (lane == 31) x_tail[warp * kTail + 5] = a4;
       __syncthreads();
       a0 += carry_in(1), a1 += carry_in(2), a2 += carry_in(3), a3 += carry_in(4);
+      if constexpr (kDepth) a4 += carry_in(5);
       int ray_next = __shfl_down_sync(0xffffffffu, ray, 1);
       if (lane == 31) ray_next = warp < 3 ? x_first[warp + 1] : -2;
       if (valid && ray_next != ray) {   // last sample of this ray inside the tile
@@ -205,9 +217,11 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
           cp[1] = a1 + (bg != nullptr ? bg[3 * ray + 1] * k : 0.f);
           cp[2] = a2 + (bg != nullptr ? bg[3 * ray + 2] * k : 0.f);
           args.comp.wsum[ray] = a3;
+          if constexpr (kDepth) args.depth[ray] = a4;
         } else {
           float* pp = args.comp.partial + ((tile_start / kTile) * 2 + (b < tile_start ? 0 : 1)) * 8;
           pp[0] = depth, pp[1] = a0, pp[2] = a1, pp[3] = a2, pp[4] = a3;
+          if constexpr (kDepth) pp[5] = a4;
         }
       }
       __syncthreads();   // the scratch words are overwritten by the next tile's operands
@@ -248,7 +262,10 @@ static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t s
   // 1.38 ms per step, 2 and 4 levels 1.40 ms.  Default 1.
   static const int unroll = [] { const char* e = getenv("HRF_FWD_UNROLL"); const int v = e ? atoi(e) : 1; return (v == 2 || v == 4) ? v : 1; }();
   int rc;
-  if (a.comp.ray_offsets != nullptr && a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true, true>);
+  if (a.comp.ray_offsets != nullptr && a.depth != nullptr && a.feat_in != nullptr)
+    rc = launch(field_forward_kernel<false, 5, false, 1, true, true, true>);
+  else if (a.comp.ray_offsets != nullptr && a.depth != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, false, true, true>);
+  else if (a.comp.ray_offsets != nullptr && a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true, true>);
   else if (a.comp.ray_offsets != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, false, true>);
   else if (a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true>);
   else if (mlp_impl != 0) rc = launch(field_forward_kernel<true, 4>);
@@ -302,6 +319,7 @@ extern "C" int hrf_field_forward(const hrf_field* f, const hrf_samples* s, int m
   a.feat_in = nullptr;
   a.feat_index = nullptr;
   a.mode = mode;
+  a.depth = nullptr;
   return launch_field_forward(a, mlp_impl, reinterpret_cast<cudaStream_t>(stream), false);
 }
 
@@ -324,6 +342,7 @@ extern "C" int hrf_field_forward_from_features(const hrf_field* f, const hrf_sam
   a.feat_in = reinterpret_cast<const uint4*>(feat_in_bf16);
   a.feat_index = feat_index;
   a.mode = 1;
+  a.depth = nullptr;
   return launch_field_forward(a, 0, reinterpret_cast<cudaStream_t>(stream), s->num_samples_dev != nullptr);
 }
 
@@ -340,12 +359,13 @@ __global__ void ray_max_chunks_kernel(const int32_t* __restrict__ off, int64_t n
 
 namespace hrf {
 // Rays whose samples straddle tile borders: chain the per-tile partials front to back.  Rays without samples are pure
-// background (volume_rendering.py:144-145 with weights_sum = 0).  One thread per ray.
-__global__ void __launch_bounds__(256) composite_fixup_kernel(const Composite c, int64_t num_rays) {
+// background (volume_rendering.py:144-145 with weights_sum = 0).  One thread per ray.  ray_depth (or NULL): sum w*t_mid,
+// chained from slot 5 of the partials with the same transmittance factor as the colour; 0 for rays without samples.
+__global__ void __launch_bounds__(256) composite_fixup_kernel(const Composite c, int64_t num_rays, float* ray_depth) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= num_rays) return;
   const int b = c.ray_offsets[r], e = c.ray_offsets[r + 1];
-  float col0 = 0.f, col1 = 0.f, col2 = 0.f, w = 0.f;
+  float col0 = 0.f, col1 = 0.f, col2 = 0.f, w = 0.f, wm = 0.f;
   if (e > b) {
     const int tf = b / kTile, tl = (e - 1) / kTile;
     if (tf == tl) return;   // finished by the forward kernel
@@ -354,6 +374,7 @@ __global__ void __launch_bounds__(256) composite_fixup_kernel(const Composite c,
       const float* pp = c.partial + ((int64_t)t * 2 + (t == tf ? 1 : 0)) * 8;
       const float T = __expf(-depth);
       col0 += T * pp[1], col1 += T * pp[2], col2 += T * pp[3], w += T * pp[4];
+      if (ray_depth != nullptr) wm += T * pp[5];
       depth += pp[0];
     }
   }
@@ -361,6 +382,7 @@ __global__ void __launch_bounds__(256) composite_fixup_kernel(const Composite c,
   if (c.background != nullptr) col0 += c.background[3 * r] * k, col1 += c.background[3 * r + 1] * k, col2 += c.background[3 * r + 2] * k;
   c.color[3 * r] = col0, c.color[3 * r + 1] = col1, c.color[3 * r + 2] = col2;
   c.wsum[r] = w;
+  if (ray_depth != nullptr) ray_depth[r] = wm;
 }
 }  // namespace hrf
 
@@ -368,9 +390,10 @@ extern "C" int64_t hrf_render_fused_workspace_bytes(int64_t num_samples_capacity
   return ((num_samples_capacity + kTile - 1) / kTile) * 2 * 8 * (int64_t)sizeof(float) + 64;
 }
 
-extern "C" int hrf_render_fused(const hrf_field* f, const hrf_samples* s, const int32_t* ray_offsets, int64_t num_rays, float step,
-                                const float* background, const void* feat_in_bf16, const int32_t* feat_index, float* color,
-                                float* weights_sum, void* workspace, void* stream) {
+// hrf_render_fused (depth = NULL) and hrf_render_fused_depth.
+static int render_fused(const hrf_field* f, const hrf_samples* s, const int32_t* ray_offsets, int64_t num_rays, float step,
+                        const float* background, const void* feat_in_bf16, const int32_t* feat_index, float* color,
+                        float* weights_sum, float* depth, void* workspace, void* stream) {
   if (int rc = check_field_args(f, s, 1)) return rc;
   HRF_REQUIRE(ray_offsets != nullptr && color != nullptr && weights_sum != nullptr, "null argument");
   HRF_REQUIRE(s->ray_origins != nullptr, "hrf_render_fused needs the ray-batch form (samples sorted by ray)");
@@ -392,11 +415,27 @@ extern "C" int hrf_render_fused(const hrf_field* f, const hrf_samples* s, const 
     a.feat_in = reinterpret_cast<const uint4*>(feat_in_bf16);
     a.feat_index = feat_in_bf16 != nullptr ? feat_index : nullptr;
     a.mode = 1;
+    a.depth = depth;
     if (int rc = launch_field_forward(a, 0, st, s->num_samples_dev != nullptr)) return rc;
   }
-  composite_fixup_kernel<<<(unsigned)((num_rays + 255) / 256), 256, 0, st>>>(c, num_rays);
+  composite_fixup_kernel<<<(unsigned)((num_rays + 255) / 256), 256, 0, st>>>(c, num_rays, depth);
   HRF_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" int hrf_render_fused(const hrf_field* f, const hrf_samples* s, const int32_t* ray_offsets, int64_t num_rays, float step,
+                                const float* background, const void* feat_in_bf16, const int32_t* feat_index, float* color,
+                                float* weights_sum, void* workspace, void* stream) {
+  return render_fused(f, s, ray_offsets, num_rays, step, background, feat_in_bf16, feat_index, color, weights_sum, nullptr,
+                      workspace, stream);
+}
+
+extern "C" int hrf_render_fused_depth(const hrf_field* f, const hrf_samples* s, const int32_t* ray_offsets, int64_t num_rays,
+                                      float step, const float* background, const void* feat_in_bf16, const int32_t* feat_index,
+                                      float* color, float* weights_sum, float* depth, void* workspace, void* stream) {
+  HRF_REQUIRE(depth != nullptr, "null depth");
+  return render_fused(f, s, ray_offsets, num_rays, step, background, feat_in_bf16, feat_index, color, weights_sum, depth,
+                      workspace, stream);
 }
 
 extern "C" int64_t hrf_density_early_stop_workspace_bytes(int64_t num_rays) { return 4 * num_rays + 64; }
@@ -431,6 +470,7 @@ extern "C" int hrf_field_density_early_stop(const hrf_field* f, const hrf_sample
   a.feat_in = nullptr;
   a.feat_index = nullptr;
   a.mode = 0;
+  a.depth = nullptr;
   ray_max_chunks_kernel<<<(unsigned)((num_rays + 255) / 256), 256, 0, st>>>(ray_offsets, num_rays,
                                                                            reinterpret_cast<int32_t*>(ws + 16));
   HRF_CHECK_LAUNCH();

@@ -158,6 +158,17 @@ class TileShardedRenderer:
     def render_range(self, cam: dict, start: int, end: int, background: float = 0.0) -> torch.Tensor:
         """cam: dict of the per-image sampler tables for ONE image (frame_numbers, camera_numbers, grid handle,
         landscape, inverse_krs, camera_origins, aabb, G, width, height).  Returns float32 [end-start, 3]."""
+        return self._render(cam, start, end, background, False)
+
+    @torch.no_grad()
+    def render_range_maps(self, cam: dict, start: int, end: int, background: float = 0.0):
+        """``render_range`` plus opacity and distance maps (hrf_render_fused_depth): returns (color [P,3], alpha [P],
+        distance [P]), P = end - start.  alpha is the weights sum; distance = sum w * t_mid / alpha, the expected
+        distance along the ray in the loader's normalised scene units, where alpha > 0, and 0 elsewhere.  Pixels outside
+        the ray mask get alpha = distance = 0.  The colours are bit-identical to ``render_range``'s."""
+        return self._render(cam, start, end, background, True)
+
+    def _render(self, cam: dict, start: int, end: int, background: float, maps: bool):
         import ctypes as C
 
         from . import _lib as L
@@ -166,7 +177,7 @@ class TileShardedRenderer:
 
         dev = cam["aabb"].device
         lib, nat, step = L.lib(), self.model.native(), self.step
-        parts = []
+        parts, alphas, dists = [], [], []
         empty_rgba = torch.zeros((0, 4), dtype=torch.uint8, device=dev)
         empty_mask = torch.zeros(0, dtype=torch.bool, device=dev)
         candidates = 0
@@ -181,6 +192,9 @@ class TileShardedRenderer:
             candidates += n
             if nr == 0:
                 parts.append(torch.full((e - s, 3), float(background), dtype=torch.float32, device=dev))
+                if maps:
+                    alphas.append(torch.zeros(e - s, dtype=torch.float32, device=dev))
+                    dists.append(torch.zeros(e - s, dtype=torch.float32, device=dev))
                 continue
             ri = rel.long()
             off0 = ray_offsets(ri, nr)
@@ -195,14 +209,22 @@ class TileShardedRenderer:
             L.check(lib.hrf_prune(sigma.data_ptr(), dist_.data_ptr(), ri.data_ptr(), off0.data_ptr(), nr, step, 1e-4, 1e-4,
                                   keep.data_ptr(), kept_off.data_ptr(), t2.data_ptr(), ri2.data_ptr(), src.data_ptr(),
                                   count.data_ptr(), L.stream()))
-            color, _ = render_fused(self.model, o, d, fn, t2, ri2, nr, float(background), step, reuse=(saved, src, kept_off),
-                                    count_dev=count)
+            out = render_fused(self.model, o, d, fn, t2, ri2, nr, float(background), step, reuse=(saved, src, kept_off),
+                               count_dev=count, want_depth=maps)
+            color = out[0]
             # combine_rays_to_image (volume_rendering.py:26-39) on the device, without nonzero(): ray j of the compacted
             # batch is the (j+1)-th set bit of the mask
             pos = (torch.cumsum(mask.view(-1).long(), 0) - 1).clamp_(min=0)
             parts.append(torch.where(mask.view(-1, 1), color[pos], torch.full((1, 3), float(background), device=dev)))
+            if maps:
+                alpha, wm = out[1].view(-1), out[2].view(-1)
+                dist = torch.where(alpha > 0, wm / alpha, torch.zeros_like(alpha))
+                m = mask.view(-1)
+                alphas.append(torch.where(m, alpha[pos], torch.zeros((), device=dev)))
+                dists.append(torch.where(m, dist[pos], torch.zeros((), device=dev)))
         self.last_stats = {"candidate_samples": candidates}
-        return parts[0] if len(parts) == 1 else torch.cat(parts, 0)
+        cat = lambda xs: xs[0] if len(xs) == 1 else torch.cat(xs, 0)
+        return (cat(parts), cat(alphas), cat(dists)) if maps else cat(parts)
 
     def render_image_sharded(self, cam: dict, rank: int, world: int, background: float = 0.0):
         """This rank's tile of the image: returns (start, end, colours)."""

@@ -197,12 +197,28 @@ def _background_rows(background, num_rays: int, dev) -> "torch.Tensor | None":
 
 
 @torch.no_grad()
+def render_with_depth(input_batch: InputBatch, scene_representation: HumanRF, background_rgb: torch.Tensor,
+                      render_step_size: float = 4e-4):
+    """``render`` without gradients (evaluation mode), plus the depth of every ray: (RenderOutput, depth [R,1]) with
+    depth = sum_i w_i * (t_start_i + t_end_i) / 2 over the samples the colour is composited from (unnormalised: divide by
+    weights_sum for the expected distance; 0 for rays without samples).  The colour and weights sum are bit-identical to
+    ``render``'s; like ``render`` it reuses the features of a preceding ``prune_samples`` of the same batch."""
+    ib = input_batch
+    o, d, fr, t, ri = _ray_arrays(ib)
+    color, wsum, depth = render_fused(scene_representation, o, d, fr, t, ri, ib.num_rays, background_rgb,
+                                      render_step_size, reuse=_reusable_features(ib, scene_representation),
+                                      want_depth=True)
+    return RenderOutput(color=color, weights_sum=wsum), depth
+
+
+@torch.no_grad()
 def render_fused(model: HumanRF, o, d, fr, t, ri, num_rays: int, background, step: float = 4e-4, cams=None, reuse=None,
-                 count_dev=None, ray_offsets_dev=None):
+                 count_dev=None, ray_offsets_dev=None, want_depth: bool = False):
     """Inference render of a ray batch in one field kernel (hrf_render_fused): encode -> MLPs -> compositing, nothing per
     sample written to HBM.  reuse = (features [M,32] bf16, row index per sample, ray-offset table) from a pruning pass:
     no encode at all.  count_dev: live sample count on the device (t / ri are then capacity-sized).
-    Returns (color [R,3], weights_sum [R,1])."""
+    Returns (color [R,3], weights_sum [R,1]); with `want_depth` (hrf_render_fused_depth) also depth [R,1] = sum w * t_mid,
+    and color / weights_sum are bit-identical to the ones without it."""
     nat = model.native()
     dev = t.device
     lib = L.lib()
@@ -216,6 +232,12 @@ def render_fused(model: HumanRF, o, d, fr, t, ri, num_rays: int, background, ste
     wsum = torch.empty((num_rays, 1), dtype=torch.float32, device=dev)
     bg = _background_rows(background, num_rays, dev)
     ws = torch.empty(int(lib.hrf_render_fused_workspace_bytes(t.shape[0])), dtype=torch.uint8, device=dev)
+    if want_depth:
+        depth = torch.empty((num_rays, 1), dtype=torch.float32, device=dev)
+        L.check(lib.hrf_render_fused_depth(C.byref(nat.field), C.byref(samples), off.data_ptr(), num_rays, float(step),
+                                           L.ptr(bg), L.ptr(feat), L.ptr(src), color.data_ptr(), wsum.data_ptr(),
+                                           depth.data_ptr(), ws.data_ptr(), L.stream()))
+        return color, wsum, depth
     L.check(lib.hrf_render_fused(C.byref(nat.field), C.byref(samples), off.data_ptr(), num_rays, float(step), L.ptr(bg),
                                  L.ptr(feat), L.ptr(src), color.data_ptr(), wsum.data_ptr(), ws.data_ptr(), L.stream()))
     return color, wsum

@@ -182,6 +182,15 @@ int hrf_render_fused(const hrf_field* f, const hrf_samples* s /* ray-batch form 
                      int64_t num_rays, float step, const float* background /* [R,3] or NULL */, const void* feat_in_bf16,
                      const int32_t* feat_index, float* color /* [R,3] */, float* weights_sum /* [R] */, void* workspace,
                      void* stream);
+/* hrf_render_fused plus a depth map, with the same inputs, workspace and rules.  For each ray r, over exactly the samples
+ * its colour is composited from, in order: depth[r] = sum_i w_i * m_i with m_i = __fmul_rn(0.5f, __fadd_rn(t_i,
+ * __fadd_rn(t_i, step))), nerfacc's (t_starts + t_ends) / 2, i.e. accumulate_along_rays(weights, values=t_mid).  It is
+ * unnormalised (depth / weights_sum is the expected distance along the ray direction), has no background term, and is 0
+ * for rays without samples.  color and weights_sum are bit-identical to what hrf_render_fused writes. */
+int hrf_render_fused_depth(const hrf_field* f, const hrf_samples* s /* ray-batch form */, const int32_t* ray_offsets /* [R+1] */,
+                           int64_t num_rays, float step, const float* background /* [R,3] or NULL */, const void* feat_in_bf16,
+                           const int32_t* feat_index, float* color /* [R,3] */, float* weights_sum /* [R] */,
+                           float* depth /* [R], non-NULL */, void* workspace, void* stream);
 
 /* Density-only pass of prune_samples (volume_rendering.py:66-84) with an exact early stop: ray chunks are
  * evaluated front to back; once a ray's accumulated optical depth makes every later sample fail nerfacc's
