@@ -749,8 +749,11 @@ int hrf_launch_scatter_v4(const hrf_field* f, const hrf_samples* s, const hrf_se
 int hrf_launch_scatter_v5(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads, const void* grid_feat_bf16,
                           const int32_t* feat_index, int64_t grid_feat_stride, const void* workspace, int grid_first, int grid_count,
                           cudaStream_t st);   // scatter_v5.cu
+int hrf_launch_scatter_v6(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads, const void* grid_feat_bf16,
+                          const int32_t* feat_index, int64_t grid_feat_stride, const void* workspace, int grid_first, int grid_count,
+                          cudaStream_t st);   // scatter_v6.cu
 #ifndef HRF_SCATTER_DEFAULT
-#define HRF_SCATTER_DEFAULT 5   // the fastest generation on the train bench on an H100 (DESIGN.md section 3.3)
+#define HRF_SCATTER_DEFAULT 6   // the fastest generation on the train bench on an H100 (DESIGN.md section 3.3)
 #endif
 
 extern "C" int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads,
@@ -760,9 +763,13 @@ extern "C" int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* 
   HRF_REQUIRE(grid_first >= 0 && grid_count >= 1 && grid_first + grid_count <= 4, "grids are 0..3 (xyz, xyt, yzt, xzt)");
   if (s->num_samples == 0) return 0;
   HRF_REQUIRE(workspace != nullptr, "needs the workspace hrf_field_backward_mlp filled");
-  // HRF_SCATTER = 5 | 4 | 3 | 2 | 1 (read per call: the tests switch it): scatter_v5.cu ... scatter_v2.cu, the
-  // first-generation kernels below.  All stay built: each is the others' cross-check in tests/test_scatter_gpu.py.
-  const int gen = [] { const char* e = getenv("HRF_SCATTER"); const int v = e ? atoi(e) : HRF_SCATTER_DEFAULT; return (v >= 1 && v <= 5) ? v : HRF_SCATTER_DEFAULT; }();
+  // HRF_SCATTER = 6 | 5 | 4 | 3 | 2 | 1 (read per call: the tests switch it): scatter_v6.cu ... scatter_v2.cu, the
+  // first-generation kernels below.  All stay built: each is the others' cross-check in tests/test_scatter_gpu.py and
+  // tests/test_scatter_v6_gpu.py.
+  const int gen = [] { const char* e = getenv("HRF_SCATTER"); const int v = e ? atoi(e) : HRF_SCATTER_DEFAULT; return (v >= 1 && v <= 6) ? v : HRF_SCATTER_DEFAULT; }();
+  if (gen == 6)
+    return hrf_launch_scatter_v6(f, s, seg_grads, grid_feat_bf16, feat_index, grid_feat_stride, workspace, grid_first, grid_count,
+                                 reinterpret_cast<cudaStream_t>(stream));
   if (gen == 5)
     return hrf_launch_scatter_v5(f, s, seg_grads, grid_feat_bf16, feat_index, grid_feat_stride, workspace, grid_first, grid_count,
                                  reinterpret_cast<cudaStream_t>(stream));

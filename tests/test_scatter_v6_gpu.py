@@ -1,0 +1,157 @@
+"""The sixth-generation table / vector gradient scatter (csrc/scatter_v6.cu, HRF_SCATTER=6) against float64 autograd
+through the oracle's hash-grid encoding and tensor composition at 1e-5 (the bar of test_scatter_gpu.py), and against v5.
+
+v6 walks all grids of a launch inside one CTA, so the cases are the ones its loop structure can get wrong: the saved
+per-grid features read through a survivor index (egrid + feat_index, a column stride wider than the sample count) and the
+re-gather path (egrid = NULL); one launch over the 4 grids and four one-grid launches (the overlapped exchange's
+schedule); full-size tables with one and with three temporal segments; samples outside a dense level's grid (the cold
+path); and a sample count that is not a multiple of the 1024 samples of a CTA."""
+import ctypes as C
+
+import numpy as np
+import pytest
+import torch
+
+from helpers import make_pair, positions_of, synthetic_rays
+from humanrf_b200 import _lib as L
+from oracle import hashgrid
+
+pytestmark = pytest.mark.gpu
+GRID_AXES = ([0, 1, 2], [0, 1, 3], [1, 2, 3], [0, 2, 3])     # xyz, xyt, yzt, xzt (decomposition4d.py:126-129)
+VECTOR_OF_GRID = (3, 2, 0, 1)                                 # xyz*v_t, xyt*v_z, yzt*v_x, xzt*v_y (tensor_composition.cu:49-52)
+CONFIGS = {"seg50": (50,), "seg100-100-50": (100, 100, 50)}
+
+
+def _relnorm(a, b):
+    a, b = a.double().reshape(-1), b.double().reshape(-1)
+    return float((a - b).norm() / b.norm().clamp_min(1e-30))
+
+
+def _lerp_vectors(vectors, coords):
+    """oracle.field.lerp_vectors with both taps clamped to the rows, as the kernels' make_tap does (coordinates outside
+    [0, 1] reach the vectors here)."""
+    vr = vectors.shape[1]
+    out = []
+    for i in range(4):
+        c = coords[:, i] * vr - 0.5
+        f = torch.floor(c)
+        frac = (c - f).unsqueeze(1)
+        i0 = torch.clamp(f, 0.0, vr - 1).long()
+        i1 = torch.clamp(f + 1, 0.0, vr - 1).long()
+        v0, v1 = vectors[i][i0], vectors[i][i1]
+        out.append(v0 + frac * (v1 - v0))
+    return torch.stack(out, 0)
+
+
+def _bf16_bits(x):
+    return (x.float().bfloat16().view(torch.int16).numpy().astype(np.int64) & 0xFFFF).astype(np.uint32)
+
+
+@pytest.fixture(scope="module", params=list(CONFIGS), ids=list(CONFIGS))
+def case(request, cuda):
+    segs = CONFIGS[request.param]
+    om, m, frames = make_pair(segs, table_std=0.5, bf16=False, device=cuda)
+    with torch.no_grad():                                      # bf16-representable tables: the re-gather path reads the bf16 shadows
+        for s, fg in enumerate(m.feature_grids):
+            for k, g in enumerate(fg.grids()):
+                q = g.detach().bfloat16().float()
+                g.copy_(q)
+                om.segments[s].grids[k] = q.cpu().reshape(-1, 2).clone()
+    nat = m.native()
+    nat.refresh()
+    b = synthetic_rays(72, 96, frames, ragged=True, seed=31)
+    pos, fr = positions_of(b), b["frames"][b["ri"]]
+    # samples outside the dense levels' grids (x beyond 1 or below 0 after the +0.5): the kernels' cold path
+    g = torch.Generator().manual_seed(4)
+    pick = torch.randint(0, pos.shape[0], (96,), generator=g)
+    out_pos = pos[pick].clone()
+    out_pos[:48, 0] = 0.5 + 0.005 + 0.03 * torch.rand(48, generator=g)
+    out_pos[48:, 0] = -0.5 - 0.02 - 0.03 * torch.rand(48, generator=g)
+    pos, fr = torch.cat((pos, out_pos)), torch.cat((fr, fr[pick]))
+    if pos.shape[0] % 1024 == 0:
+        pos, fr = pos[:-1], fr[:-1]
+    n = pos.shape[0]
+    assert n > 2048 and n % 1024 != 0
+    seg = om.f2s[fr.numpy()]
+    if len(segs) > 1:
+        assert len(np.unique(seg)) > 1
+    xyzt = torch.cat((pos + 0.5, torch.from_numpy(om.f2t[fr.numpy()]).unsqueeze(1)), dim=1).float()
+    d_out = torch.randn(n, 32, generator=g)
+    d_out[::7] = 0                                            # zero upstream gradients are skipped, not scattered
+
+    # ---- reference: float64 autograd.  Table gradients do not depend on the features; the vector gradients of the
+    # egrid path use the saved bf16 features, those of the re-gather path the exact blend of the (bf16) tables.
+    ref_tables, ref_vec_gather, ref_vec_egrid = [], [], []
+    enc_all = torch.zeros(n, 4, 32, dtype=torch.float64)
+    for s, sd in enumerate(om.segments):
+        sel = torch.from_numpy(np.nonzero(seg == s)[0])
+        tabs = [t.double().requires_grad_(True) for t in sd.grids]
+        c = xyzt[sel]
+        enc = [hashgrid.encode(tabs[k], c[:, GRID_AXES[k]], sd.log2T) for k in range(4)]
+        for k in range(4):
+            enc_all[sel, k] = enc[k].detach()
+        saved = [e.detach().float().bfloat16().double() for e in enc]
+        vg = sd.vectors.double().requires_grad_(True)
+        ve = sd.vectors.double().requires_grad_(True)
+        sv_g, sv_e = _lerp_vectors(vg, c), _lerp_vectors(ve, c)
+        out_g = sum(enc[k] * sv_g[VECTOR_OF_GRID[k]] for k in range(4))
+        out_e = sum(saved[k] * sv_e[VECTOR_OF_GRID[k]] for k in range(4))
+        (((out_g + out_e) * d_out[sel].double()).sum()).backward()
+        ref_tables.append([t.grad.reshape(-1) if t.grad is not None else torch.zeros(t.numel(), dtype=torch.float64) for t in tabs])
+        ref_vec_gather.append(vg.grad if vg.grad is not None else torch.zeros_like(vg))
+        ref_vec_egrid.append(ve.grad if ve.grad is not None else torch.zeros_like(ve))
+
+    # saved per-(level, grid) features [16 * 4][stride] bf16x2, each sample at a shuffled column of a wider buffer
+    stride = n + 37
+    perm = torch.randperm(stride, generator=g)[:n]
+    bits = _bf16_bits(enc_all)                                                 # [n, 4, 32]
+    packed = bits[..., 0::2] | (bits[..., 1::2] << np.uint32(16))             # [n, 4 grids, 16 levels]
+    egrid = np.zeros((64, stride), np.uint32)
+    egrid[:, perm.numpy()] = packed.transpose(2, 1, 0).reshape(64, n)
+    dev = {"egrid": torch.from_numpy(egrid.view(np.int32)).to(cuda), "feat_index": perm.to(torch.int32).to(cuda)}
+
+    ws = torch.zeros(n * 40, dtype=torch.float32, device=cuda)
+    ws[: 32 * n] = d_out.reshape(n, 16, 2).permute(1, 0, 2).reshape(-1).to(cuda)
+    ws[32 * n: 36 * n] = xyzt.reshape(-1).to(cuda)
+    ws.view(torch.uint8)[144 * n: 145 * n] = torch.from_numpy(seg.astype(np.uint8)).to(cuda)
+    samples = nat.samples_query(pos.to(cuda).contiguous(), None, fr.to(cuda).to(torch.int32).contiguous())
+    return dict(m=m, nat=nat, samples=samples, ws=ws, stride=stride, dev=dev, ref_tables=ref_tables,
+                ref_vec={"gather": ref_vec_gather, "egrid": ref_vec_egrid})
+
+
+def _run(case, monkeypatch, gen, mode, launches):
+    monkeypatch.setenv("HRF_SCATTER", gen)
+    m, nat = case["m"], case["nat"]
+    grads = [torch.zeros_like(p) for p in m.hot_parameters()]
+    sg = (L.SegmentGrads * m.num_segments)()
+    for s in range(m.num_segments):
+        for k in range(4):
+            sg[s].grid[k] = grads[5 * s + k].data_ptr()
+        sg[s].vectors = grads[5 * s + 4].data_ptr()
+    sg_dev = torch.from_numpy(np.frombuffer(bytes(sg), dtype=np.uint8).copy()).to(grads[0].device)
+    eg, fi, stride = (case["dev"]["egrid"].data_ptr(), case["dev"]["feat_index"].data_ptr(), case["stride"]) if mode == "egrid" else (None, None, 0)
+    for first, count in ([(0, 4)] if launches == "one" else [(k, 1) for k in range(4)]):
+        L.check(L.lib().hrf_field_backward_tables(C.byref(nat.field), C.byref(case["samples"]), sg_dev.data_ptr(), eg, fi, stride,
+                                                  case["ws"].data_ptr(), first, count, L.stream()))
+    torch.cuda.synchronize()
+    return [g.cpu() for g in grads]
+
+
+@pytest.mark.parametrize("launches", ["one", "four"], ids=["grid_count4", "4x_grid_count1"])
+@pytest.mark.parametrize("mode", ["egrid", "gather"], ids=["egrid+feat_index", "regather"])
+def test_scatter_v6_matches_float64_autograd_and_v5(cuda, monkeypatch, case, mode, launches):
+    got6 = _run(case, monkeypatch, "6", mode, launches)
+    got5 = _run(case, monkeypatch, "5", mode, "one")
+    for s in range(len(case["ref_tables"])):
+        for k in range(4):
+            g6, g5, ref = got6[5 * s + k], got5[5 * s + k], case["ref_tables"][s][k]
+            assert ((g6 != 0) & (ref == 0)).sum() == 0, "gradient written to an untouched table entry"
+            e = _relnorm(g6, ref)
+            worst = float((g6.double() - ref).abs().max() / ref.abs().max().clamp_min(1e-30))
+            e5 = _relnorm(g6, g5)
+            print(f"{mode} {launches} seg{s} grid{k}: relnorm {e:.2e} worst entry {worst:.2e} vs v5 {e5:.2e} touched {(ref != 0).sum().item()}")
+            assert e < 1e-5 and worst < 1e-5 and e5 < 1e-5
+        ev = _relnorm(got6[5 * s + 4], case["ref_vec"][mode][s])
+        ev5 = _relnorm(got6[5 * s + 4], got5[5 * s + 4])
+        print(f"{mode} {launches} seg{s} vectors: relnorm {ev:.2e} vs v5 {ev5:.2e}")
+        assert ev < 1e-5 and ev5 < 1e-5
