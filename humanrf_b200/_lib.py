@@ -118,6 +118,8 @@ _SIGNATURES = {
     "hrf_marching_cubes_workspace_bytes": (i64, [C.c_int]),
     "hrf_marching_cubes_count": (C.c_int, [vp, C.c_int, f32, vp, vp, vp]),
     "hrf_marching_cubes_emit": (C.c_int, [vp, C.c_int, f32, i64, i64, vp, vp, vp, vp, vp]),
+    "hrf_image_metrics_workspace_bytes": (i64, [C.c_int, C.c_int]),
+    "hrf_image_metrics": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

@@ -456,6 +456,29 @@ int hrf_marching_cubes_emit(const float* lattice, int grid_resolution, float lev
                             int32_t* faces /* [F,3] */, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Image scores of the ActorsHQ evaluation (actorshq/evaluation/evaluate.py:76-85,117-125) on one pair of 8-bit images.
+ * pred, gt: uint8 [H*W*3] RGB, row-major pixels; mask: uint8 [H*W], non-zero = foreground.
+ *   ROI : cv2.boundingRect of the pixels with mask != 0, written as roi = {x, y, w, h}; {0, 0, 0, 0} for an empty mask.
+ *   PSNR: out[0] = -10 log10(MSE), MSE = sum over masked pixels of sum_c (p_c - g_c)^2 / (3 * 255^2 * masked count);
+ *         the sum is exact (int64), the log fp64.  MSE = 0 gives +inf.
+ *   SSIM: out[1] = scikit-image's structural_similarity(gt_roi, pred_roi, channel_axis=2) with its defaults for uint8
+ *         (data_range 255, 7x7 uniform window, K1 0.01, K2 0.03, sample covariance vx = 49/48 (E[x^2] - E[x]^2)):
+ *         S = (2 ux uy + C1)(2 vxy + C2) / ((ux^2 + uy^2 + C1)(vx + vy + C2)), C1 = (0.01*255)^2, C2 = (0.03*255)^2,
+ *         averaged over the windows lying wholly inside the ROI (skimage's crop of 3 pixels on every side; its
+ *         reflect-mode border never reaches them), then over the 3 channels.  Window sums are exact int32, S is fp64.
+ *   NaN : SSIM when the ROI is narrower or shorter than 7 pixels (scikit-image raises there); both for an empty mask.
+ * Image bytes are read as the aligned 32-bit words containing them.  Nothing here synchronises: out / roi may be rows
+ * of larger device arrays that are read back once after many calls.  Partial sums are folded in a fixed order, so two
+ * calls write identical bytes.  width * height * 3 < 2^31.  workspace: hrf_image_metrics_workspace_bytes(width, height)
+ * bytes of device scratch, 16-byte aligned.
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_image_metrics_workspace_bytes(int width, int height);
+int hrf_image_metrics(const uint8_t* pred /* [H*W*3] RGB */, const uint8_t* gt /* [H*W*3] RGB */,
+                      const uint8_t* mask /* [H*W], non-zero = foreground */, int width, int height,
+                      double* out /* [2] device: PSNR (dB), SSIM */, int32_t* roi /* [4] device: x, y, w, h */,
+                      void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
