@@ -161,14 +161,19 @@ class TileShardedRenderer:
         return self._render(cam, start, end, background, False)
 
     @torch.no_grad()
-    def render_range_maps(self, cam: dict, start: int, end: int, background: float = 0.0):
+    def render_range_maps(self, cam: dict, start: int, end: int, background: float = 0.0, normals: bool = False):
         """``render_range`` plus opacity and distance maps (hrf_render_fused_depth): returns (color [P,3], alpha [P],
         distance [P]), P = end - start.  alpha is the weights sum; distance = sum w * t_mid / alpha, the expected
         distance along the ray in the loader's normalised scene units, where alpha > 0, and 0 elsewhere.  Pixels outside
-        the ray mask get alpha = distance = 0.  The colours are bit-identical to ``render_range``'s."""
-        return self._render(cam, start, end, background, True)
+        the ray mask get alpha = distance = 0.  The colours are bit-identical to ``render_range``'s.
 
-    def _render(self, cam: dict, start: int, end: int, background: float, maps: bool):
+        With `normals`, a fourth output [P,3]: unit normals in normalised scene coordinates, N / |N| with
+        N = sum_i w_i n_i over the same samples and weights, n_i = -grad sigma_i / |grad sigma_i| (0 where the gradient
+        vanishes; hrf_field_position_grad).  0 where |N| = 0 and outside the ray mask.  Colour, alpha and distance are
+        bit-identical to the call without normals."""
+        return self._render(cam, start, end, background, True, normals)
+
+    def _render(self, cam: dict, start: int, end: int, background: float, maps: bool, normals: bool = False):
         import ctypes as C
 
         from . import _lib as L
@@ -177,7 +182,7 @@ class TileShardedRenderer:
 
         dev = cam["aabb"].device
         lib, nat, step = L.lib(), self.model.native(), self.step
-        parts, alphas, dists = [], [], []
+        parts, alphas, dists, norms, nwsums = [], [], [], [], []
         empty_rgba = torch.zeros((0, 4), dtype=torch.uint8, device=dev)
         empty_mask = torch.zeros(0, dtype=torch.bool, device=dev)
         candidates = 0
@@ -195,6 +200,9 @@ class TileShardedRenderer:
                 if maps:
                     alphas.append(torch.zeros(e - s, dtype=torch.float32, device=dev))
                     dists.append(torch.zeros(e - s, dtype=torch.float32, device=dev))
+                if normals:
+                    norms.append(torch.zeros((e - s, 3), dtype=torch.float32, device=dev))
+                    nwsums.append(torch.zeros(e - s, dtype=torch.float32, device=dev))
                 continue
             ri = rel.long()
             off0 = ray_offsets(ri, nr)
@@ -222,9 +230,45 @@ class TileShardedRenderer:
                 m = mask.view(-1)
                 alphas.append(torch.where(m, alpha[pos], torch.zeros((), device=dev)))
                 dists.append(torch.where(m, dist[pos], torch.zeros((), device=dev)))
+            if normals:
+                nrm, nws = self._normals(nat, o, d, fn, t2, ri2, count, saved, src, kept_off, nr)
+                norms.append(torch.where(mask.view(-1, 1), nrm[pos], torch.zeros((), device=dev)))
+                nwsums.append(torch.where(mask.view(-1), nws[pos], torch.zeros((), device=dev)))
         self.last_stats = {"candidate_samples": candidates}
         cat = lambda xs: xs[0] if len(xs) == 1 else torch.cat(xs, 0)
+        if normals:
+            # the weights sum of the normals' compositing pass, per pixel: a check that it composited what the render did
+            self.last_stats["normal_weights_sum"] = cat(nwsums)
+            return cat(parts), cat(alphas), cat(dists), cat(norms)
         return (cat(parts), cat(alphas), cat(dists)) if maps else cat(parts)
+
+    def _normals(self, nat, o, d, fn, t2, ri2, count, saved, src, kept_off, nr):
+        """Unit normal per compacted ray of one batch, from the survivors of its prune pass.  The survivor buffers are
+        capacity-sized and only the first `count` (a device scalar) rows are live: every step below honours the live
+        count or reads through `kept_off`, nothing indexes them on the host side.  Returns (normals [R,3], weights sum [R])."""
+        import ctypes as C
+
+        from . import _lib as L
+
+        lib, dev, n = L.lib(), t2.device, t2.shape[0]
+        samples = nat.samples_rays(o, d, fn, t2, ri2, count_dev=count)
+        sigma, _ = nat.forward_from_features(samples, saved, src)
+        ws = torch.empty(n * 40, dtype=torch.float32, device=dev)     # 160 B / sample, hrf_field_backward_mlp's layout
+        ones = torch.ones(n, dtype=torch.float32, device=dev)
+        L.check(lib.hrf_field_backward_mlp(C.byref(nat.field), C.byref(samples), ones.data_ptr(), None, None, saved.data_ptr(),
+                                           src.data_ptr(), None, None, ws.data_ptr(), L.stream()))
+        grad = torch.zeros((n, 3), dtype=torch.float32, device=dev)
+        L.check(lib.hrf_field_position_grad(C.byref(nat.field), C.byref(samples), ws.data_ptr(), grad.data_ptr(), L.stream()))
+        gn = torch.linalg.vector_norm(grad, dim=1, keepdim=True)
+        n_i = torch.where(gn > 0, -grad / torch.where(gn > 0, gn, torch.ones_like(gn)), torch.zeros_like(grad))
+        acc = torch.empty((nr, 3), dtype=torch.float32, device=dev)
+        wsum = torch.empty(nr, dtype=torch.float32, device=dev)
+        # sum_i w_i n_i with the render's weights: the compositing kernel with the normals in place of the colours and no
+        # background term
+        L.check(lib.hrf_composite_forward(sigma.data_ptr(), n_i.data_ptr(), t2.data_ptr(), kept_off.data_ptr(), nr, self.step,
+                                          None, acc.data_ptr(), wsum.data_ptr(), None, L.stream()))
+        an = torch.linalg.vector_norm(acc, dim=1, keepdim=True)
+        return torch.where(an > 0, acc / torch.where(an > 0, an, torch.ones_like(an)), torch.zeros_like(acc)), wsum
 
     def render_image_sharded(self, cam: dict, rank: int, world: int, background: float = 0.0):
         """This rank's tile of the image: returns (start, end, colours)."""

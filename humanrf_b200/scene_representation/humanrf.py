@@ -117,8 +117,13 @@ class HumanRF(torch.nn.Module):
 
     # ------------------------------------------------------------------ reference API
     def density(self, query_input: QueryInput) -> QueryOutput:
-        needs_grad = self._needs_grad()
-        active = self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers) if needs_grad else None
+        """sigma and the geometry features.  When ``query_input.positions`` requires grad, the backward also returns
+        d(positions) [N,3] (hrf_field_position_grad): the exact derivative of what the kernels compute, grid and vector
+        terms both, with the bf16 rounding of the composed features treated as the identity.  Not covered: gradients of
+        the directions, first-order only (``create_graph=True`` is not supported)."""
+        needs_grad = self._needs_grad(query_input.positions)
+        active = (self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers)
+                  if self._needs_grad() else None)
         sigma, geo, _ = _FieldFunction.apply(self, 0, query_input.positions, None, query_input.frame_numbers, None,
                                              needs_grad, active, *self.hot_parameters())
         return QueryOutput(density=sigma, geometry_features=geo)
@@ -126,8 +131,10 @@ class HumanRF(torch.nn.Module):
     def forward(self, query_input: QueryInput) -> QueryOutput:
         # humanrf.py:194-204: the camera embedding is looked up while training and is all zeros otherwise
         cams = query_input.camera_numbers if (self.camera_embedding_dim > 0 and query_input.is_training) else None
-        needs_grad = self._needs_grad()
-        active = self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers) if needs_grad else None
+        # d(positions) as in density(); the radiance reaches the positions through the geometry features
+        needs_grad = self._needs_grad(query_input.positions)
+        active = (self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers)
+                  if self._needs_grad() else None)
         sigma, geo, rgb = _FieldFunction.apply(self, 1, query_input.positions, query_input.directions,
                                                query_input.frame_numbers, cams, needs_grad, active, *self.hot_parameters())
         return QueryOutput(density=sigma, geometry_features=geo, radiance=rgb)
@@ -143,9 +150,12 @@ class HumanRF(torch.nn.Module):
         src = unique_frame_numbers if unique_frame_numbers is not None else frame_numbers
         return active_segments(self.frame_numbers_to_segment_numbers, src, self.num_segments).cpu().tolist()
 
-    def _needs_grad(self) -> bool:
-        # ctx.needs_input_grad ignores torch.no_grad(); decide outside whether to save the backward buffers
-        return torch.is_grad_enabled() and any(p.requires_grad for p in self.hot_parameters())
+    def _needs_grad(self, positions: Optional[torch.Tensor] = None) -> bool:
+        # ctx.needs_input_grad ignores torch.no_grad(); decide outside whether to save the backward buffers.  Positions
+        # that require grad count too: their gradient needs the same saved features.
+        if not torch.is_grad_enabled():
+            return False
+        return (positions is not None and positions.requires_grad) or any(p.requires_grad for p in self.hot_parameters())
 
     def get_params(self, lr):
         params = [
@@ -389,9 +399,11 @@ class _NativeField:
         return sigma if save == "none" else (sigma, saved)
 
     def backward(self, samples: L.Samples, d_sigma, d_rgb, feat, grad_tensors: List[torch.Tensor], per_table: bool = False,
-                 d_geo=None, feat_index=None):
+                 d_geo=None, feat_index=None, d_positions: Optional[torch.Tensor] = None):
         """grad_tensors: fp32 buffers in hot_parameters() order (accumulated into).  per_table launches the scatter once
-        per grid instead of once for all four.  d_geo: fp32 [N,15] gradient of the geometry features, or None."""
+        per grid instead of once for all four.  d_geo: fp32 [N,15] gradient of the geometry features, or None.
+        d_positions: fp32 [N,3] written with the position gradient (hrf_field_position_grad, after the scatter, on the
+        same workspace: the parameter gradients are the launches without it), or None."""
         m = self.model
         dev = self._device()
         sg = (L.SegmentGrads * m.num_segments)()
@@ -420,9 +432,30 @@ class _NativeField:
             L.check(L.lib().hrf_field_backward(C.byref(self.field), C.byref(samples), sg_dev.data_ptr(), L.ptr(d_sigma),
                                                L.ptr(d_rgb), L.ptr(d_geo), L.ptr(feat), egrid, L.ptr(feat_index), 0, d_mlp.data_ptr(),
                                                L.ptr(d_emb), ws.data_ptr(), L.stream()))
+        if d_positions is not None:
+            L.check(L.lib().hrf_field_position_grad(C.byref(self.field), C.byref(samples), ws.data_ptr(), d_positions.data_ptr(),
+                                                    L.stream()))
         grad_tensors[i].add_(d_mlp[:MLP_SIGMA_PARAMS])
         grad_tensors[i + 1].add_(d_mlp[MLP_SIGMA_PARAMS:])
         return sg_dev  # keep alive until the kernel has run (stream-ordered free is safe, but be explicit)
+
+    def position_backward(self, samples: L.Samples, d_sigma, d_rgb, feat, d_geo=None, feat_index=None,
+                          d_positions: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The position gradient alone, for frozen parameters: the MLP backward (its weight gradients go to a scratch
+        buffer that is dropped) and hrf_field_position_grad on its workspace; no table scatter.  Returns d_positions
+        fp32 [N,3] (rows past a device-side live count are left as they were: zeros when allocated here)."""
+        dev = self._device()
+        n = int(samples.num_samples)
+        d_mlp = torch.empty(self.model.mlp_grad_elems, dtype=torch.float32, device=dev)
+        ws = torch.empty(n * 40, dtype=torch.float32, device=dev)   # 160 B / sample
+        if d_positions is None:
+            d_positions = torch.zeros((n, 3), dtype=torch.float32, device=dev)
+        lib = L.lib()
+        L.check(lib.hrf_field_backward_mlp(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb), L.ptr(d_geo),
+                                           L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(), None, ws.data_ptr(), L.stream()))
+        L.check(lib.hrf_field_position_grad(C.byref(self.field), C.byref(samples), ws.data_ptr(), d_positions.data_ptr(),
+                                            L.stream()))
+        return d_positions
 
 
 def _as_f32c(t: torch.Tensor) -> torch.Tensor:
@@ -451,6 +484,7 @@ class _FieldFunction(torch.autograd.Function):
         ctx.save_for_backward(pos, dirs if dirs is not None else pos, frames, feat if feat is not None else pos,
                               cams if cams is not None else frames)
         ctx.has_dirs, ctx.has_cams = dirs is not None, cams is not None
+        ctx.pos_dtype, ctx.pos_shape = positions.dtype, positions.shape
         geo_out = geo[:, 1:]            # differentiable: humanrf.py:185-186 hands sigma_net's outputs 1..15 to the caller
         if rgb is None:
             rgb = sigma.new_zeros((0, 3))
@@ -463,17 +497,27 @@ class _FieldFunction(torch.autograd.Function):
         pos, dirs, frames, feat, cams = ctx.saved_tensors
         nat = model.native()
         params = model.hot_parameters()
-        grads = [torch.zeros_like(p) for p in params]
         samples = nat.samples_query(pos, dirs if ctx.has_dirs else None, frames, cams if ctx.has_cams else None)
         ds = None if d_sigma is None else _as_f32c(d_sigma)
         dr = None if (d_rgb is None or ctx.mode == 0) else _as_f32c(d_rgb)
         if ds is None:
             ds = torch.zeros(pos.shape[0], dtype=torch.float32, device=pos.device)
         dg = None if d_geo is None else _as_f32c(d_geo)
-        keep = nat.backward(samples, ds, dr, feat, grads, d_geo=dg)
+        want_pos = ctx.needs_input_grad[2]
+        d_pos = torch.empty((pos.shape[0], 3), dtype=torch.float32, device=pos.device) if want_pos else None
+        if not any(ctx.needs_input_grad[8:]):
+            if not want_pos:
+                return (None,) * (8 + len(params))
+            # every parameter frozen: the MLP backward and the position kernel only, no table scatter
+            nat.position_backward(samples, ds, dr, feat, d_geo=dg, d_positions=d_pos)
+            d_pos_out = d_pos.to(ctx.pos_dtype).reshape(ctx.pos_shape)
+            return (None, None, d_pos_out, None, None, None, None, None, *([None] * len(params)))
+        grads = [torch.zeros_like(p) for p in params]
+        keep = nat.backward(samples, ds, dr, feat, grads, d_geo=dg, d_positions=d_pos)
         del keep
         if ctx.active is not None:      # segments the batch did not touch get no gradient at all (None), as in the reference
             from ..parallel import mask_inactive_segment_grads
 
             grads = mask_inactive_segment_grads(grads, ctx.active)
-        return (None, None, None, None, None, None, None, None, *grads)
+        d_pos_out = None if d_pos is None else d_pos.to(ctx.pos_dtype).reshape(ctx.pos_shape)
+        return (None, None, d_pos_out, None, None, None, None, None, *grads)

@@ -74,7 +74,8 @@ class _Views:
     def hull(self, frame: int) -> torch.Tensor:
         return torch.from_numpy(np.ascontiguousarray(self.loader.dataset.get_occupancy_grid(frame_number=frame))).to(self.device)
 
-    def render(self, camera_number: int, frame: int, grid: torch.Tensor) -> DepthMap:
+    def tables(self, camera_number: int, frame: int, grid: torch.Tensor) -> dict:
+        """The renderer's per-image tables of one view (``TileShardedRenderer.render_range``'s `cam`)."""
         from ..dataset.occupancy_grid_native import OccupanyGrid
 
         dl, dev = self.loader, self.device
@@ -94,6 +95,12 @@ class _Views:
                       inverse_krs=dl.all_inverse_krs[camera_number:camera_number + 1].contiguous(),
                       camera_origins=dl.all_camera_origins[camera_number:camera_number + 1].contiguous(),
                       aabb=dl.aabb, G=self.G, width=W, height=H)
+        return tables
+
+    def render(self, camera_number: int, frame: int, grid: torch.Tensor) -> DepthMap:
+        dl = self.loader
+        tables = self.tables(camera_number, frame, grid)
+        W, H = tables["width"], tables["height"]
         color, alpha, dist = self.renderer.render_range_maps(tables, 0, W * H, 0.0)
         scale = float(dl.scene_scale)
         norms = pixel_ray_norms(dl.all_inverse_krs[camera_number], W, H)

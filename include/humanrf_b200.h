@@ -268,6 +268,17 @@ int hrf_field_backward_mlp(const hrf_field* f, const hrf_samples* s, const float
 int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads,
                               const void* grid_feat_bf16, const int32_t* feat_index, int64_t grid_feat_stride,
                               const void* workspace, int grid_first, int grid_count, void* stream);
+/* Position gradient: d_positions[i] = sum over levels l and grids k of J_{k,l}(p_i)^T . dF_l(i), the derivative of the
+ * composed features hrf_field_forward computes, contracted with d(composed features).  `workspace` is what
+ * hrf_field_backward_mlp filled for the same `s`: dF as float2 [16][N] at 0, normalised positions at 128 N, segment ids
+ * at 144 N (N = s->num_samples).  J includes both the grid term (the corner weights' derivative, scaled by the level
+ * scale; a grid's time dimension feeds no position component) and the vector term e_k * vec_res * (v[i1] - v[i0]) of
+ * the one grid whose vector runs along the axis (0 where the tap clamps).  The bf16 rounding of the features before the
+ * MLP counts as the identity.  Written, not accumulated, for i < live count (s->num_samples_dev honoured); rows past
+ * the live count are untouched; rows of samples whose frame has no segment are 0.  Query and ray-batch form.  No
+ * atomics: two runs write identical bytes.  Nothing here synchronises. */
+int hrf_field_position_grad(const hrf_field* f, const hrf_samples* s, const void* workspace,
+                            float* d_positions /* [N,3] */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Training loss on the per-ray outputs, forward and backward in one launch (trainer.py:205-215,229-238,
