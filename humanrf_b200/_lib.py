@@ -55,6 +55,10 @@ class AdamTensor(C.Structure):
                 ("active", vp), ("step", vp), ("n", i64), ("first_block", i64), ("vectors_t", vp), ("vec_res", i32)]
 
 
+class LpipsWeights(C.Structure):
+    _fields_ = [("packed", vp), ("bias", vp * 5), ("lin", vp * 5)]
+
+
 ADAM_BLOCK_ELEMS = 4096
 DP_MAX_WORLD = 8
 
@@ -121,6 +125,10 @@ _SIGNATURES = {
     "hrf_marching_cubes_emit": (C.c_int, [vp, C.c_int, f32, i64, i64, vp, vp, vp, vp, vp]),
     "hrf_image_metrics_workspace_bytes": (i64, [C.c_int, C.c_int]),
     "hrf_image_metrics": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp]),
+    "hrf_lpips_packed_bytes": (i64, []),
+    "hrf_lpips_pack_weights": (C.c_int, [C.POINTER(vp), vp, vp]),
+    "hrf_lpips_workspace_bytes": (i64, [C.c_int, C.c_int]),
+    "hrf_lpips": (C.c_int, [C.POINTER(LpipsWeights), vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

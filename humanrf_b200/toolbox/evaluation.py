@@ -5,7 +5,7 @@ include/humanrf_b200.h): a PSNR over the mask's pixels and scikit-image's SSIM o
 numbers ``actorshq/evaluation/evaluate.py`` writes.  ``evaluate_sequence`` replaces the reference's ``Trainer.test`` +
 ``evaluate`` pair: it renders each (camera, frame) view, scores it against the dataset's image and mask without the image
 leaving the device, optionally writes the 8-bit PNGs ``Trainer.test`` writes, and writes ``metrics.csv`` and
-``averages.csv``.  LPIPS and VMAF are not computed.
+``averages.csv``.  LPIPS is added when weights are given (toolbox/lpips.py); VMAF is not computed.
 """
 from __future__ import annotations
 
@@ -21,16 +21,19 @@ from .. import _lib as L
 from .depth_maps import _check_camera, _check_frame, _Views, camera_name
 
 METRICS = ("PSNR", "SSIM")
+METRICS_LPIPS = ("PSNR", "LPIPS", "SSIM")     # evaluate.py's order
 
 
 @dataclass
 class ViewScore:
-    """Scores of one view: camera number (0-based), frame, PSNR (dB), SSIM and the ROI (x, y, w, h)."""
+    """Scores of one view: camera number (0-based), frame, PSNR (dB), SSIM, the ROI (x, y, w, h) and LPIPS (None when
+    not computed)."""
     camera: int
     frame: int
     psnr: float
     ssim: float
     roi: tuple
+    lpips: float | None = None
 
 
 def _check_image(t, name, shape):
@@ -107,22 +110,31 @@ def write_frame_png(path, rgb_u8) -> None:
 
 def write_metric_tables(out_dir, scores) -> None:
     """``metrics.csv`` (camera numbered from 1, frame, PSNR, SSIM per view, in order) and ``averages.csv`` (the mean of
-    each metric), laid out as actorshq/evaluation/evaluate.py writes them, without its LPIPS column."""
+    each metric), laid out as actorshq/evaluation/evaluate.py writes them.  Its LPIPS column, between PSNR and SSIM, is
+    written when every score carries an LPIPS."""
+    with_lpips = bool(scores) and all(s.lpips is not None for s in scores)
+    metrics = METRICS_LPIPS if with_lpips else METRICS
     os.makedirs(out_dir, exist_ok=True)
     with open(os.path.join(out_dir, "metrics.csv"), "w", newline="") as f:
-        w = csv.DictWriter(f, fieldnames=["camera", "frame", *METRICS])
+        w = csv.DictWriter(f, fieldnames=["camera", "frame", *metrics])
         w.writeheader()
         for s in scores:
-            w.writerow({"camera": s.camera + 1, "frame": s.frame, "PSNR": s.psnr, "SSIM": s.ssim})
+            row = {"camera": s.camera + 1, "frame": s.frame, "PSNR": s.psnr, "SSIM": s.ssim}
+            if with_lpips:
+                row["LPIPS"] = s.lpips
+            w.writerow(row)
     with open(os.path.join(out_dir, "averages.csv"), "w", newline="") as f:
-        w = csv.DictWriter(f, fieldnames=list(METRICS))
+        w = csv.DictWriter(f, fieldnames=list(metrics))
         w.writeheader()
-        w.writerow({"PSNR": float(np.mean([s.psnr for s in scores])), "SSIM": float(np.mean([s.ssim for s in scores]))})
+        row = {"PSNR": float(np.mean([s.psnr for s in scores])), "SSIM": float(np.mean([s.ssim for s in scores]))}
+        if with_lpips:
+            row["LPIPS"] = float(np.mean([s.lpips for s in scores]))
+        w.writerow(row)
 
 
 @torch.no_grad()
 def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_frames: bool = True,
-                      render_step_size: float = 4e-4, rays_per_batch: int = 262144):
+                      render_step_size: float = 4e-4, rays_per_batch: int = 262144, lpips_weights=None):
     """Renders every (camera_number, frame_number) of `pairs` with `model` through `loader`'s cameras (the colour of
     ``render_depth_map``), quantises it to 8 bits as ``Trainer.test`` does and scores it against the dataset's image and
     mask with ``image_metrics``.  With `save_frames` the views are written as ``out_dir/test_frames/<cam>_rgb%06d.png``
@@ -130,16 +142,19 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
     ``out_dir/metrics.csv`` and ``out_dir/averages.csv``.  Views are rendered from the dataset's hulls, as the reference's
     evaluation loader does; with `bake` each frame's hull is first tightened by ``bake_occupancy_grid`` (once per
     frame).  Cameras and frames are checked before anything is written; the scores are read back once, at the end, and
-    a view without a score (empty mask, or an ROI under 7x7 pixels) raises before the tables are written.  Returns a
-    ``ViewScore`` per pair."""
+    a view without a score (empty mask, or an ROI under 7x7 pixels) raises before the tables are written.  With
+    `lpips_weights` (``load_lpips_alex``) each view's LPIPS is computed too, on the quantised render against the dataset
+    image over the ROI ``image_metrics`` wrote, and the tables gain evaluate.py's LPIPS column; an ROI under 31x31 pixels
+    has no LPIPS and raises.  Returns a ``ViewScore`` per pair."""
     from .learned_occupancy import bake_occupancy_grid
+    from .lpips import lpips
 
     pairs = [(_check_camera(loader, c), _check_frame(model, f)) for c, f in pairs]
     if not pairs:
         raise RuntimeError("no (camera, frame) pairs to evaluate")
     views = _Views(model, loader, render_step_size, rays_per_batch)
     dev = views.device
-    values = torch.empty(len(pairs), 2, dtype=torch.float64, device=dev)
+    values = torch.empty(len(pairs), 2 if lpips_weights is None else 3, dtype=torch.float64, device=dev)
     rois = []
     grids = {}
     if save_frames:
@@ -150,15 +165,22 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
             grids[frame] = bake_occupancy_grid(model, frame, grid, render_step_size) if bake else grid
         pred = quantize(views.render(c, frame, grids[frame]).color)
         gt, mask = ground_truth(loader, c, frame)
-        _, roi = image_metrics(pred, torch.from_numpy(gt).to(dev), torch.from_numpy(mask).to(dev), out=values[k])
+        gt = torch.from_numpy(gt).to(dev)
+        _, roi = image_metrics(pred, gt, torch.from_numpy(mask).to(dev), out=values[k, :2])
+        if lpips_weights is not None:
+            lpips(pred, gt, lpips_weights, roi=roi, out=values[k, 2])
         rois.append(roi)
         if save_frames:
             write_frame_png(frame_path(out_dir, camera_name(loader, c), frame), pred)
     v = values.cpu().numpy()
     r = torch.stack(rois).cpu().numpy()
-    scores = [ViewScore(c, f, float(v[k, 0]), float(v[k, 1]), tuple(int(x) for x in r[k])) for k, (c, f) in enumerate(pairs)]
+    scores = [ViewScore(c, f, float(v[k, 0]), float(v[k, 1]), tuple(int(x) for x in r[k]),
+                        None if lpips_weights is None else float(v[k, 2])) for k, (c, f) in enumerate(pairs)]
     bad = [(s.camera, s.frame) for s in scores if math.isnan(s.psnr) or math.isnan(s.ssim)]
     if bad:
         raise RuntimeError(f"no score for (camera, frame) {bad}: empty mask, or a mask bounding box under 7x7 pixels")
+    bad = [(s.camera, s.frame) for s in scores if s.lpips is not None and math.isnan(s.lpips)]
+    if bad:
+        raise RuntimeError(f"no LPIPS for (camera, frame) {bad}: a mask bounding box under 31x31 pixels")
     write_metric_tables(out_dir, scores)
     return scores

@@ -490,6 +490,53 @@ int hrf_image_metrics(const uint8_t* pred /* [H*W*3] RGB */, const uint8_t* gt /
                       void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * LPIPS of the ActorsHQ evaluation and the reference trainer's checkpoint choice (evaluate.py:66-73,
+ * trainer.py:408-412): lpips.LPIPS(net="alex", version="0.1") called with normalize=True on the ROI crop of both images.
+ *   Input: pred, gt [H*W*3] RGB, row-major pixels, dtype 0 = uint8 (v = u / 255.0f, correctly rounded), 1 = float32
+ *          (v as given).  roi = device int32 {x, y, w, h} (e.g. what hrf_image_metrics writes), or NULL for the whole
+ *          image.  Then x = 2v - 1 and x = (x - shift) / scale in fp32 with IEEE division, shift = (-.030, -.088, -.188),
+ *          scale = (.458, .448, .450) as fp32 values of those literals, channels in RGB order.
+ *   Trunk: torchvision's alexnet().features[0:12]: conv1 3->64 11x11/4 pad 2, ReLU, maxpool 3/2, conv2 64->192 5x5
+ *          pad 2, ReLU, maxpool 3/2, conv3 192->384 3x3 pad 1, ReLU, conv4 384->256, ReLU, conv5 256->256, ReLU (3x3
+ *          pad 1).  The five ReLU outputs are the LPIPS layers.  The convolutions are implicit GEMMs on TF32 wgmma:
+ *          every operand is rounded to tf32 explicitly (cvt.rna: nearest, ties away from zero), the activations in the
+ *          epilogue that writes them (after bias and ReLU) and the input after the scaling above, the weights once when
+ *          packed, so the MMA's own truncation changes nothing.  Accumulation, bias and ReLU are fp32.
+ *   Tail : per layer k and pixel, f = y / (sqrt(sum_c y^2) + 1e-10) for each image, d = sum_c lin_k[c] (f0 - f1)^2, all
+ *          fp32; d is averaged over the layer's H x W (spatial sums folded in fp64) and out[0] = the sum of the five
+ *          means (fp64).  This is torch's own precision class: cuDNN convolutions use TF32 by default on Ampere and
+ *          later GPUs.
+ *   NaN  : out[0] when the ROI is narrower or shorter than 31 pixels (torch raises there: pool2 would be empty), which
+ *          includes the empty-mask ROI {0, 0, 0, 0}, and when it does not lie inside the image.
+ * No floating-point atomics, every fold in a fixed order: two calls (and a CUDA-graph replay) write identical bytes,
+ * swapping pred and gt gives identical bytes and identical images give exactly 0.  Nothing here synchronises: grids
+ * are sized from width x height and CTAs outside the ROI exit.  width * height * 3 < 2^31.
+ *
+ * Weights: hrf_lpips_pack_weights packs torchvision's five OIHW fp32 conv weights (features.{0,3,6,8,10}.weight) into
+ * hrf_lpips_packed_bytes() bytes of device memory (16-byte aligned); the layout is private to the library.  bias[k]
+ * (features.*.bias) and lin[k] (lpips' lin{k}.model.1.weight, flattened) are fp32 device arrays of 64, 192, 384, 256 and
+ * 256 values.
+ *
+ * workspace: hrf_lpips_workspace_bytes(width, height) bytes of device scratch, 256-byte aligned; about 1.6 GB at
+ * 4112x3008 (sized for ROI = whole image).  It holds eight fp32 NHWC tensors, each [2][h][w][C] with image 0 = pred and
+ * image 1 = gt and (h, w) the tensor's size for the ROI: input (C = 4, the 4th channel zero), conv1 (64), pool1 (64),
+ * conv2 (192), pool2 (192), conv3 (384), conv4 (256), conv5 (256).  Tensor i starts at byte offset
+ * sum_{j<i} roundup(2 * H_j * W_j * C_j * 4, 256), with H_j x W_j its size for the whole image; the tail's fp64 per-CTA
+ * sums follow.  Sizes: conv1 (n - 7) / 4 + 1, each pool (n - 3) / 2 + 1, every other layer keeps its input's size.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct hrf_lpips_weights {
+  const void* packed;    /* hrf_lpips_packed_bytes() bytes written by hrf_lpips_pack_weights */
+  const float* bias[5];  /* conv biases, device fp32 */
+  const float* lin[5];   /* lin weights, device fp32 */
+} hrf_lpips_weights;
+int64_t hrf_lpips_packed_bytes(void);
+int hrf_lpips_pack_weights(const float* const* conv_w /* [5] device pointers, OIHW fp32 */, void* packed, void* stream);
+int64_t hrf_lpips_workspace_bytes(int width, int height);
+int hrf_lpips(const hrf_lpips_weights* weights, const void* pred, const void* gt, int dtype /* 0 uint8, 1 float32 */,
+              int width, int height, const int32_t* roi /* device x, y, w, h, or NULL */,
+              double* out /* [1] device */, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
