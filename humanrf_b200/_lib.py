@@ -129,6 +129,9 @@ _SIGNATURES = {
     "hrf_lpips_pack_weights": (C.c_int, [C.POINTER(vp), vp, vp]),
     "hrf_lpips_workspace_bytes": (i64, [C.c_int, C.c_int]),
     "hrf_lpips": (C.c_int, [C.POINTER(LpipsWeights), vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
+    "hrf_mesh_distance_workspace_bytes": (i64, [i64, i64, i64, C.c_int]),
+    "hrf_mesh_distance": (C.c_int, [vp, i64, vp, i64, vp, i64, vp, i64, i64, u64, C.POINTER(f32), C.c_int, vp, vp, vp,
+                                    vp, vp, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

@@ -537,6 +537,46 @@ int hrf_lpips(const hrf_lpips_weights* weights, const void* pred, const void* gt
               double* out /* [1] device */, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Surface distance of one direction between two triangle meshes (DESIGN.md §3.11; restated in numpy in
+ * tests/geometry_oracle.py): N points sampled on the source S by area, each queried against the target T.  Vertices
+ * fp32 [V*3], faces int32 [F*3], both meshes in the same units.  u = round-to-nearest fp32 operations, each rounded on
+ * its own (no FMA contraction).
+ *   Eligible face: indices in [0, V) and 0 < |n|^2 < inf for n = e1 x e2, e1 = v1 - v0, e2 = v2 - v0,
+ *          n = (e1.y e2.z - e1.z e2.y, e1.z e2.x - e1.x e2.z, e1.x e2.y - e1.y e2.x), |n|^2 = (n.x^2 + n.y^2) + n.z^2.
+ *          Ineligible faces are never sampled and never a target.  area = 0.5 sqrt(|n|^2), n^ = n / sqrt(|n|^2).
+ *   Sampling: q_f = floor(area_f / area_max * 2^32) (uint64; division in fp64; area_max = largest eligible area;
+ *          q_f = 0 when ineligible), P = exclusive prefix sum of q, Q = sum of q.  Sample k (0 <= k < N) draws
+ *          x_j = splitmix64(seed * 2^40 + 3k + j), j = 0, 1, 2 (uint64 arithmetic; splitmix64(x): z = x +
+ *          0x9E3779B97F4A7C15, z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9, z = (z ^ z >> 27) * 0x94D049BB133111EB,
+ *          z ^ z >> 31).  Its face is the f with P_f <= mulhi64(x_0, Q) < P_f + q_f; u1 = (x_1 >> 40) 2^-24,
+ *          u2 = (x_2 >> 40) 2^-24, r = sqrt(u1), w0 = 1 - r, w1 = r (1 - u2), w2 = r u2 and per component
+ *          p = (w0 v0 + w1 v1) + w2 v2.
+ *   Distance: d2(p, t) = Ericson's closest point on a triangle (Real-Time Collision Detection §5.1.5) in fp32, its
+ *          point clamped per component into the triangle's bounding box, then |p - q|^2 = (e.x^2 + e.y^2) + e.z^2.
+ *          closest = the eligible target face of least d2, the lowest face id on ties; d = sqrt(d2).  Both equal a
+ *          brute-force scan bit for bit (the tree prunes a node only when a lower bound, rounded down, is strictly
+ *          greater than the best d2 so far).  Normal term: |n^_S(face_k) . n^_T(closest)|.
+ *   Scores: out = {sum d, sum d^2, sum normal term} / N in fp64 (d^2 of the fp32 d, exact in fp64), partial sums per
+ *          CTA folded in a fixed order; counts[i] = #{k : d_k <= taus[i]} (fp32 comparison), num_taus <= 8.
+ *          out = NaN and counts = -1 when *error != 0, when S or T has no eligible face (Q = 0), or F = 0.
+ *   error: device int32, bit 0 = a source face index outside [0, V), bit 1 = a target one; such faces are ineligible
+ *          and their vertices are never read.
+ * Optional per-sample outputs (device, nullable): points [N*3], sample_faces [N], distances [N] (+inf when T has no
+ * eligible face, NaN when S has none) and closest_faces [N] (-1 when none).  No floating-point atomics, no host
+ * synchronisation: two calls (and a CUDA-graph replay) write identical bytes.  F < 2^31, 1 <= N < 2^31.  taus is a host
+ * array.  workspace: hrf_mesh_distance_workspace_bytes(F_src, F_tgt, N, num_taus) bytes of device scratch (0 = bad
+ * sizes), 256-byte aligned.
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_mesh_distance_workspace_bytes(int64_t num_src_faces, int64_t num_tgt_faces, int64_t num_samples,
+                                          int num_taus);
+int hrf_mesh_distance(const float* src_vertices, int64_t num_src_vertices, const int32_t* src_faces,
+                      int64_t num_src_faces, const float* tgt_vertices, int64_t num_tgt_vertices,
+                      const int32_t* tgt_faces, int64_t num_tgt_faces, int64_t num_samples, uint64_t seed,
+                      const float* taus /* host [num_taus] */, int num_taus, double* out /* [3] device */,
+                      int64_t* counts /* [num_taus] device */, int32_t* error /* [1] device */, float* points,
+                      int32_t* sample_faces, float* distances, int32_t* closest_faces, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
