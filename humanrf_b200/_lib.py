@@ -132,6 +132,12 @@ _SIGNATURES = {
     "hrf_mesh_distance_workspace_bytes": (i64, [i64, i64, i64, C.c_int]),
     "hrf_mesh_distance": (C.c_int, [vp, i64, vp, i64, vp, i64, vp, i64, i64, u64, C.POINTER(f32), C.c_int, vp, vp, vp,
                                     vp, vp, vp, vp, vp, vp]),
+    "hrf_rasterize_mesh_workspace_bytes": (i64, [i64, i64, C.c_int, C.c_int]),
+    "hrf_rasterize_mesh": (C.c_int, [vp, i64, vp, i64, C.POINTER(C.c_double), C.c_double, C.c_double, C.c_double,
+                                     C.c_double, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp, vp, vp, vp,
+                                     vp]),
+    "hrf_depth_metrics_workspace_bytes": (i64, [i64]),
+    "hrf_depth_metrics": (C.c_int, [vp, vp, vp, vp, i64, C.POINTER(C.c_double), C.c_int, vp, vp, vp, vp, vp]),
     "hrf_selftest_umma": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, u32, u32, u32, u32, u32, u32, u32, u32,
                                     C.c_int, vp]),
 }

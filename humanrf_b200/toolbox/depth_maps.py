@@ -4,7 +4,8 @@
 variant, include/humanrf_b200.h ``hrf_render_fused_depth``) and converts the expected ray distance into the camera-space
 depth along the optical axis, in world units: the quantity the ActorsHQ toolbox's mesh renderer writes
 (``depth = position_cam.z`` with an RDF camera, 0 on background).  ``export_depth_sequence`` writes those maps and the
-thresholded opacity in that renderer's file layout, so the two sets of outputs can be compared file by file.
+thresholded opacity in that renderer's file layout.  ``toolbox/mesh_depth.py`` writes the dataset meshes' maps in the
+same layout (``export_mesh_depth_sequence``) and scores the two against each other (``evaluate_depth``).
 
 Unlike a mesh (``toolbox/mesh_extraction.py``) the depth needs no iso-level: it is the weight-averaged distance of what
 the model renders, pixel for pixel aligned with its colour image.

@@ -577,6 +577,65 @@ int hrf_mesh_distance(const float* src_vertices, int64_t num_src_vertices, const
                       int32_t* sample_faces, float* distances, int32_t* closest_faces, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Mesh rasterisation into a depth map and a mask: the outputs of the ActorsHQ toolbox's mesh renderer
+ * (mesh_tools/renderer: camera-space z of an RDF camera, GL_LESS, no culling, 0 on background), deterministic and
+ * exact (DESIGN.md §3.12; restated in numpy in tests/raster_oracle.py).  Vertices fp32 [V*3], faces int32 [F*3].
+ * world2cam = host fp64 [12], row-major 3x4 (the host takes (inv(cam2world) diag(s, s, s, 1))[:3] in fp64); fxW, fyH,
+ * cxW, cyH = focal length and principal point in pixels, the principal point measured from the image's corner.  Every
+ * fp64 operation below is rounded to nearest on its own (no contraction).
+ *   1 Vertex: p in fp64; X = ((m00 p.x + m01 p.y) + m02 p.z) + m03, Y and Z likewise with rows 1 and 2;
+ *          u = (fxW X) / Z + cxW, v = (fyH Y) / Z + cyH; U = rint(256 u), V = rint(256 v) (ties to even) as integers.
+ *          A vertex is out when !(near <= Z <= DBL_MAX) or !(|256 u| <= 2^29 and |256 v| <= 2^29) (NaN included).
+ *   2 Faces that draw nothing (their vertices are never read, or read only for the check): a face with an index
+ *          outside [0, V) (sets error bit 0); a face with a vertex out (a documented divergence from GL, which clips;
+ *          counted in *skipped); a face with A = (U1 - U0)(V2 - V0) - (V1 - V0)(U2 - U0) = 0; a face whose clipped box
+ *          is empty: pixel columns ceil((min U - 128) / 256) .. floor((max U - 128) / 256) within [0, width), rows
+ *          likewise within [0, height).
+ *   3 Coverage: pixel (x, y) (column x, row y, row 0 at the top) samples S = (256 x + 128, 256 y + 128), the pixel
+ *          centre.  Edge k runs from vertex k+1 to vertex k+2 (indices mod 3), d_k = v_{k+2} - v_{k+1},
+ *          E_k = sgn(A) (d_k.x (S.y - v_{k+1}.y) - d_k.y (S.x - v_{k+1}.x)), exact in int64 (every product < 2^60), so
+ *          E_0 + E_1 + E_2 = |A| and both windings draw.  S is covered when for every k: E_k > 0, or E_k = 0 and
+ *          P(sgn(A) d_k) with P(d) = d.y > 0 or (d.y = 0 and d.x < 0).  P(d) != P(-d): of two faces on opposite sides
+ *          of a shared edge exactly one covers a sample on it, and a closed fan covers its centre once.
+ *   4 Depth: b_k = (double)E_k / (double)|A|, z = (float)(1 / ((b_0 / Z_0 + b_1 / Z_1) + b_2 / Z_2)): the
+ *          perspective-correct camera z of the face's plane along the pixel's ray.  A covered sample is a fragment
+ *          when near <= z <= far (z as fp64).
+ *   5 Visibility: each pixel keeps the least key (float bits of z) << 32 | face over its fragments: the nearest
+ *          face, on equal z the lowest face id (GL_LESS in draw order).  Integer atomics only: two calls (and a
+ *          CUDA-graph replay) write identical bytes.
+ * Outputs [height*width], row-major: z fp32 (0 without a fragment), mask uint8 (255 / 0), face int32 (-1; nullable),
+ * hits int32 (the number of faces of step 3 that cover the pixel centre, before the near / far test; nullable).
+ * error: device int32, bit 0 as above.  skipped: device int64.  No host synchronisation.  F < 2^31,
+ * width * height < 2^31, 0 < near <= far < inf.  workspace: hrf_rasterize_mesh_workspace_bytes(V, F, width, height)
+ * bytes of device scratch (0 = bad sizes), 256-byte aligned; O(V + F + width * height).
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_rasterize_mesh_workspace_bytes(int64_t num_vertices, int64_t num_faces, int width, int height);
+int hrf_rasterize_mesh(const float* vertices, int64_t num_vertices, const int32_t* faces, int64_t num_faces,
+                       const double* world2cam /* host [12] */, double fxW, double fyH, double cxW, double cyH,
+                       int width, int height, double near, double far, float* z, uint8_t* mask, int32_t* face,
+                       int32_t* hits, int32_t* error /* [1] device */, int64_t* skipped /* [1] device */,
+                       void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Depth and mask scores of a depth map against a reference (DESIGN.md §3.12).  pred_z, ref_z fp32 [N]; pred_mask,
+ * ref_mask uint8 [N], non-zero = foreground.  B = pixels where both masks are set; for a pixel of B,
+ * d = (double)pred - (double)ref (rounded to nearest).  Per CTA in fp64, folded by one CTA in a fixed order:
+ *   out[0] = sum d / n (bias), out[1] = sum |d| / n (MAE), out[2] = sqrt(sum d^2 / n) (RMSE),
+ *   out[3] = sum (|d| / ref) / n (AbsRel), n = |B|;
+ *   counts (int64) = {n, |P|, |R|, |P and R|, |P or R|, #{|d| <= taus[i]} for i < num_taus (fp64 comparison)}.
+ * A pixel of B with a z on either side that is not finite and > 0 sets error bit 0 and is left out of the sums.
+ * out = NaN when *error != 0 or n = 0; counts are always written.  No floating-point atomics, no host synchronisation
+ * (out and counts may be rows of larger arrays): two calls write identical bytes.  1 <= N < 2^31, num_taus <= 8, taus
+ * a host array.  workspace: hrf_depth_metrics_workspace_bytes(N) bytes of device scratch (0 = bad size), 16-byte
+ * aligned.
+ * ---------------------------------------------------------------------------------------- */
+int64_t hrf_depth_metrics_workspace_bytes(int64_t num_pixels);
+int hrf_depth_metrics(const float* pred_z, const uint8_t* pred_mask, const float* ref_z, const uint8_t* ref_mask,
+                      int64_t num_pixels, const double* taus /* host [num_taus] */, int num_taus,
+                      double* out /* [4] device */, int64_t* counts /* [5 + num_taus] device */,
+                      int32_t* error /* [1] device */, void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
