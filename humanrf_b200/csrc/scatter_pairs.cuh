@@ -1,6 +1,19 @@
 // The lane-pair walk of the table / vector gradient scatter (scatter_v5.cu, scatter_v6.cu): what one warp does for one
-// (level, grid) over the 128 samples it has staged in shared memory.  See scatter_v5.cu for why the parity slots are
-// split over the two lanes of a pair.  v5 and v6 differ only in what a CTA covers and how it stages its inputs.
+// (level, grid) over the 128 samples it has staged in shared memory.  v5 and v6 differ only in what a CTA covers and how
+// it stages its inputs.
+//
+// Consecutive samples of a ray mostly stay in the same cell or step into a neighbouring one, so the walk accumulates
+// w * g per vertex over a run of samples and issues one RED per run, not per sample.  The accumulators are PARITY SLOTS:
+// indexed not by corner offset (dx, dy, dz) but by the parity of the vertex coordinate on each axis.  A cell [g, g+1]
+// holds exactly one even and one odd vertex per axis, so
+//   * when the ray steps into the neighbouring cell along an axis, the vertex the two cells share keeps its slot and its
+//     accumulator (that is the shared-corner carry), and the vertex that enters has the parity of the one that leaves,
+//     so it takes over that slot.  "Flush and zero the slots whose table index changed" is the whole carry: no data
+//     moves between slots, and jumps and new rays need no special case;
+//   * "index changed" is one integer compare per slot and a flush is a predicated RED; the corner weights are computed
+//     in slot order directly (two selects per axis).  The per-sample step is straight-line code, with no divergent
+//     branch for the runs.
+// The 8 slots of a sample are split over the two lanes of a pair by the parity of the first-axis vertex (scatter_v5.cu).
 #pragma once
 
 #include <cstddef>
@@ -26,21 +39,9 @@ struct ScatterV5Args {
 };
 
 __device__ __forceinline__ void red2v5(float* addr, float a, float b) {
+  // No "memory" clobber: the scatter never reads the gradient buffers, and the clobber would pin every load of the next
+  // step behind this step's REDs.
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b));
-}
-
-struct RowTap5 {
-  uint32_t i0, i1;
-  float frac;
-};
-__device__ __forceinline__ RowTap5 make_row_tap5(float coord, int vec_res) {
-  const float c = __fmaf_rn(coord, (float)vec_res, -0.5f);
-  const float fl = floorf(c);
-  RowTap5 t;
-  t.frac = c - fl;
-  t.i0 = (uint32_t)min(max((int)fmaxf(fl, 0.f), 0), vec_res - 1);
-  t.i1 = (uint32_t)min(max((int)fminf(fl + 1.f, (float)(vec_res - 1)), 0), vec_res - 1);
-  return t;
 }
 
 // Table entries of the 4 vertices of a cell whose FIRST-axis vertex has parity p, in parity-slot order (slot bit 0 = parity
@@ -126,7 +127,7 @@ __device__ __forceinline__ void scatter_level_pairs(const ScatterV5Args& a, cons
     uint32_t changed = 0u;
     uint32_t nidx[4] = {0u, 0u, 0u, 0u};
     Cell A{0u, 0.f}, B{0u, 0.f}, C{0u, 0.f};
-    RowTap5 tp{0u, 0u, 0.f};
+    RowTap2 tp{0u, 0u, 0.f};
     float2 dO = make_float2(0.f, 0.f);
     if (ok) {
       const float4 p4 = sm.pos[row + j];
@@ -135,7 +136,7 @@ __device__ __forceinline__ void scatter_level_pairs(const ScatterV5Args& a, cons
       const float c1 = (kGrid == 0 || kGrid == 1) ? p4.y : p4.z;
       const float c2 = (kGrid == 0) ? p4.z : p4.w;
       const float cv = (kAxis == 0) ? p4.x : (kAxis == 1) ? p4.y : (kAxis == 2) ? p4.z : p4.w;
-      tp = make_row_tap5(cv, f.vec_res);
+      tp = make_row_tap2(cv, f.vec_res);
       A = to_cell(scale, c0), B = to_cell(scale, c1), C = to_cell(scale, c2);
       if (sgi != cur_sgi) {                           // (rare) new temporal segment: flush everything, new constants
         if (gtab != nullptr) {

@@ -1,16 +1,16 @@
 // Table / vector gradient scatter, fifth generation (replaces tcnn kernel_grid_backward + compose_tensors_backward,
-// tensor_composition.cu:57-118).  Same arithmetic as scatter_v3.cu / scatter_v4.cu; the change is what ONE RED
-// INSTRUCTION carries to the L2.
+// tensor_composition.cu:57-118).  Its walk (scatter_pairs.cuh) is shaped by what ONE RED INSTRUCTION carries to the L2.
 //
-// v3 and v4, two kernels with very different SM-side pictures (issue slots, warps per SM), take about the same time,
-// and both send one RED request of ONE sector per lane to the L2.  A thread owns all vertices of its sample, so the 32 lanes of a RED instruction address 32 unrelated cells: one request
-// per lane.  But the two vertices of a cell that differ in the FIRST axis are neighbours in the table (tcnn's hash
-// multiplies the first axis by 1; a dense level is x-major): 15 times out of 16 they lie in the same 128-byte line.
-// Here the 8 parity slots of a sample chunk are split over the two lanes of a LANE PAIR by the parity of the first-axis
-// vertex, and the pair flushes a slot TOGETHER (when either lane's entry changed): both entries leave in the same RED
-// instruction and share one L2 request.  A lane that flushes early only splits its sum in two adds.
+// When a thread owns all vertices of its sample, the 32 lanes of a RED instruction address 32 unrelated cells: one L2
+// request of one sector per lane.  But the two vertices of a cell that differ in the FIRST axis are neighbours in the
+// table (tcnn's hash multiplies the first axis by 1; a dense level is x-major): 15 times out of 16 they lie in the same
+// 128-byte line.  Here the 8 parity slots of a sample chunk are split over the two lanes of a LANE PAIR by the parity of
+// the first-axis vertex, and the pair flushes a slot TOGETHER (when either lane's entry changed): both entries leave in
+// the same RED instruction and share one L2 request.  A lane that flushes early only splits its sum in two adds.
 // The vector-row gradient is split the same way: the even lane owns tap row i0, the odd lane row i1.
-// The walk of one (level, grid) is scatter_level_pairs (scatter_pairs.cuh), shared with scatter_v6.cu.
+// A CTA covers 1024 samples, one grid and half of the levels.  scatter_v6.cu walks the same way over a different CTA
+// shape and is the one the train step runs; this kernel is its reference in the tests.  DESIGN.md section 3.3 has the
+// measurements against the earlier generations.
 #include <cstdlib>
 
 #include "scatter_pairs.cuh"

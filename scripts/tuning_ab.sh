@@ -14,6 +14,5 @@ HRF_FWD_UNROLL=2 b --mode render > "$out/render_unroll2.json"
 HRF_FWD_UNROLL=4 b --mode render > "$out/render_unroll4.json"
 b --mode render > "$out/render_default_b.json"
 b > "$out/train_default_a.json"
-for g in 1 2 4 5; do HRF_SCATTER=$g b > "$out/train_scatter$g.json"; done
-HRF_SCATTER_CTAS=6 b > "$out/train_scatter3_ctas6.json"
+HRF_SCATTER=5 b > "$out/train_scatter5.json"
 b > "$out/train_default_b.json"

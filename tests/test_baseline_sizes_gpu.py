@@ -166,7 +166,7 @@ def test_backward_matches_autograd(cuda, pair, use_saved_features):
 
 
 def test_table_scatter_matches_float64_autograd(cuda, pair):
-    """grid_scatter (the default staged kernel) alone at 1e-5 against float64 autograd, on the dense and hashed levels
+    """The default table / vector gradient scatter (scatter_v6.cu) alone at 1e-5 against float64 autograd, on the dense and hashed levels
     of the full-size tables."""
     segs, om, m, frames = pair
     pos, _, fr = bench_slice(frames, segs, rays=8, per_ray=128)

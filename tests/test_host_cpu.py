@@ -111,6 +111,30 @@ def test_c_abi_exports_every_declared_symbol():
     assert _lib.lib().hrf_version() >= 1
 
 
+def test_scatter_generation_other_than_6_or_5_is_an_error(monkeypatch):
+    """HRF_SCATTER names the scatter kernel hrf_field_backward_tables runs.  A value naming no built kernel fails the
+    call instead of running the default under that name.  Checked before any device work, so an empty batch shows it."""
+    from humanrf_b200 import _lib
+
+    if not _lib.LIB_PATH.exists():
+        pytest.skip("library not built yet (python -m humanrf_b200.build)")
+    lib = _lib.lib()
+    field, samples, seg_grads = _lib.Field(), _lib.Samples(), (_lib.SegmentGrads * 1)()   # num_samples = 0
+
+    def call():
+        return lib.hrf_field_backward_tables(ctypes.byref(field), ctypes.byref(samples), ctypes.addressof(seg_grads), None, None,
+                                             0, None, 0, 4, None)
+
+    monkeypatch.delenv("HRF_SCATTER", raising=False)
+    _lib.check(call())
+    for gen in ("6", "5"):
+        monkeypatch.setenv("HRF_SCATTER", gen)
+        _lib.check(call())
+    monkeypatch.setenv("HRF_SCATTER", "3")
+    with pytest.raises(RuntimeError, match="HRF_SCATTER must be 6"):
+        _lib.check(call())
+
+
 def test_product_does_not_import_oracle():
     for p in (ROOT / "humanrf_b200").rglob("*.py"):
         src = p.read_text()

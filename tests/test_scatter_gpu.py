@@ -1,7 +1,18 @@
-"""The table / vector gradient scatter (grid_scatter_kernel) in isolation, against float64 autograd through the
-oracle's hash-grid encoding and tensor composition: the kernel's only rounding is fp32 accumulation, so the bar is
-1e-5 -- tight enough to catch a single dropped or doubled corner contribution (the run-length accumulation and the
-shared-corner carry between neighbouring cells are exactly where such a bug would sit)."""
+"""The table / vector gradient scatter (hrf_field_backward_tables) in isolation, against float64 autograd through the
+oracle's hash-grid encoding and tensor composition.  HRF_SCATTER picks the kernel: 6 = csrc/scatter_v6.cu, the one the
+train step runs; 5 = csrc/scatter_v5.cu, the same lane-pair walk (csrc/scatter_pairs.cuh) over a different CTA shape,
+kept as v6's second reference.  The kernels' only rounding is fp32 accumulation, so the bar is 1e-5 -- tight enough to
+catch a single dropped or doubled corner contribution (the run-length accumulation and the shared-corner carry between
+neighbouring cells are exactly where such a bug would sit).
+
+The ragged-ray test runs both generations on two small temporal segments, with either feature source and several splits
+of the 4 grids over launches.
+
+v6 walks all grids of a launch inside one CTA, so its own test covers the cases that loop structure can get wrong: the
+saved per-grid features read through a survivor index (egrid + feat_index, a column stride wider than the sample count)
+and the re-gather path (egrid = NULL); one launch over the 4 grids and four one-grid launches (the overlapped exchange's
+schedule); full-size tables with one and with three temporal segments; samples outside a dense level's grid (the cold
+path); and a sample count that is not a multiple of the 1024 samples of a CTA."""
 import ctypes as C
 
 import numpy as np
@@ -16,6 +27,7 @@ from oracle import hashgrid
 pytestmark = pytest.mark.gpu
 GRID_AXES = ([0, 1, 2], [0, 1, 3], [1, 2, 3], [0, 2, 3])     # xyz, xyt, yzt, xzt (decomposition4d.py:126-129)
 VECTOR_OF_GRID = (3, 2, 0, 1)                                 # xyz*v_t, xyt*v_z, yzt*v_x, xzt*v_y (tensor_composition.cu:49-52)
+CONFIGS = {"seg50": (50,), "seg100-100-50": (100, 100, 50)}
 
 
 def _relnorm(a, b):
@@ -23,31 +35,30 @@ def _relnorm(a, b):
     return float((a - b).norm() / b.norm().clamp_min(1e-30))
 
 
-@pytest.mark.parametrize("staged,carry,chunk,taps", [("v3", "5", "", "vt"), ("v5", "5", "", ""), ("v4", "5", "", ""), ("v3", "6", "", ""), ("v3", "5", "", ""), ("v2", "6", "", ""), ("v2", "5", "", ""),
-                                                     ("1", "1", "8", "0"), ("1", "1", "8", "1"), ("1", "0", "8", "1"), ("0", "1", "16", "0"),
-                                                     ("0", "0", "8", "0"), ("0", "1", "5", "0")],
-                         ids=["v3-transposed-vector-grads", "v5-lane-pairs", "v4-split-slots", "v3-warp-private", "v3-5ctas", "v2-parity-slots", "v2-5ctas", "staged", "staged-tapstage",
-                              "staged-tapstage-nocarry", "strided16", "strided8-nocarry", "strided5"])
-def test_table_scatter_matches_float64_autograd(cuda, monkeypatch, staged, carry, chunk, taps):
-    """Every generation of the scatter (HRF_SCATTER = 5 | 4 | 3 | 2 | 1): v5 = csrc/scatter_v5.cu (the parity slots split over a
-    lane pair by the parity of the first-axis vertex, pair-wide flushes), v4 = csrc/scatter_v4.cu (the 8 parity slots of a sample
-    chunk split over two threads), v3 = csrc/scatter_v3.cu (parity-slot accumulators,
-    warp-private staging, transposed vector rows), v2 = csrc/scatter_v2.cu (parity slots, block staging), staged / strided
-    = the first-generation kernels (shared-memory staging with the shifted-corner carry; the strided first kernel behind
-    HRF_SCATTER_STAGED=0)."""
-    vec_t = taps == "vt"     # v3 with the vector-row gradient accumulated in the transposed scratch + hrf_fold_vector_grads
-    if staged in ("v2", "v3", "v4", "v5"):
-        monkeypatch.setenv("HRF_SCATTER", staged[1])
-        monkeypatch.setenv("HRF_SCATTER_CTAS", carry)
-        staged, carry, chunk, taps = "1", "1", "8", "0"
-    else:
-        monkeypatch.setenv("HRF_SCATTER", "1")
-    monkeypatch.setenv("HRF_SCATTER_STAGED", staged)
-    monkeypatch.setenv("HRF_SCATTER_TAPSTAGE", taps)
-    monkeypatch.setenv("HRF_SCATTER_CARRY", carry)
-    monkeypatch.setenv("HRF_SCATTER_CHUNK", chunk)
-    om, m, frames = make_pair((6, 6), table_std=0.5, bf16=False)
-    with torch.no_grad():                                      # bf16-representable tables: the kernel re-gathers the bf16 shadows
+def _lerp_vectors(vectors, coords):
+    """oracle.field.lerp_vectors with both taps clamped to the rows, as the kernels' make_tap does (coordinates outside
+    [0, 1] reach the vectors here)."""
+    vr = vectors.shape[1]
+    out = []
+    for i in range(4):
+        c = coords[:, i] * vr - 0.5
+        f = torch.floor(c)
+        frac = (c - f).unsqueeze(1)
+        i0 = torch.clamp(f, 0.0, vr - 1).long()
+        i1 = torch.clamp(f + 1, 0.0, vr - 1).long()
+        v0, v1 = vectors[i][i0], vectors[i][i1]
+        out.append(v0 + frac * (v1 - v0))
+    return torch.stack(out, 0)
+
+
+def _bf16_bits(x):
+    return (x.float().bfloat16().view(torch.int16).numpy().astype(np.int64) & 0xFFFF).astype(np.uint32)
+
+
+def _bf16_model(segs, cuda):
+    """An oracle / module pair with bf16-representable tables: the re-gather path reads the bf16 shadows."""
+    om, m, frames = make_pair(segs, table_std=0.5, bf16=False, device=cuda)
+    with torch.no_grad():
         for s, fg in enumerate(m.feature_grids):
             for k, g in enumerate(fg.grids()):
                 q = g.detach().bfloat16().float()
@@ -55,6 +66,86 @@ def test_table_scatter_matches_float64_autograd(cuda, monkeypatch, staged, carry
                 om.segments[s].grids[k] = q.cpu().reshape(-1, 2).clone()
     nat = m.native()
     nat.refresh()
+    return om, m, nat, frames
+
+
+def _workspace(d_out, xyzt, seg, cuda):
+    """What hrf_field_backward_mlp leaves for the scatter: d(features) level-major [16][n] float2 | (x,y,z,t) [n] float4
+    | segment [n] u8."""
+    n = d_out.shape[0]
+    ws = torch.zeros(n * 40, dtype=torch.float32, device=cuda)
+    ws[: 32 * n] = d_out.reshape(n, 16, 2).permute(1, 0, 2).reshape(-1).to(cuda)
+    ws[32 * n: 36 * n] = xyzt.reshape(-1).to(cuda)
+    ws.view(torch.uint8)[144 * n: 145 * n] = torch.from_numpy(seg.astype(np.uint8)).to(cuda)
+    return ws
+
+
+def _segment_grads(m):
+    """Zeroed gradients of m.hot_parameters() and the device array of hrf_segment_grads that points into them."""
+    grads = [torch.zeros_like(p) for p in m.hot_parameters()]
+    sg = (L.SegmentGrads * m.num_segments)()
+    for s in range(m.num_segments):
+        for k in range(4):
+            sg[s].grid[k] = grads[5 * s + k].data_ptr()
+        sg[s].vectors = grads[5 * s + 4].data_ptr()
+    sg_dev = torch.from_numpy(np.frombuffer(bytes(sg), dtype=np.uint8).copy()).to(grads[0].device)
+    return grads, sg_dev
+
+
+def _reference(om, seg, xyzt, d_out, lerp):
+    """float64 autograd of sum_k encode_k * lerp(vector_k) against d_out, per segment.  Table gradients do not depend on
+    the features; the vector gradients of the egrid path use the saved bf16 features, those of the re-gather path the
+    exact blend of the (bf16) tables.  Also returns every sample's exact per-grid features [n, 4, 32]."""
+    ref_tables, ref_vec_gather, ref_vec_egrid = [], [], []
+    enc_all = torch.zeros(xyzt.shape[0], 4, 32, dtype=torch.float64)
+    for s, sd in enumerate(om.segments):
+        sel = torch.from_numpy(np.nonzero(seg == s)[0])
+        tabs = [t.double().requires_grad_(True) for t in sd.grids]
+        c = xyzt[sel]
+        enc = [hashgrid.encode(tabs[k], c[:, GRID_AXES[k]], sd.log2T) for k in range(4)]
+        for k in range(4):
+            enc_all[sel, k] = enc[k].detach()
+        saved = [e.detach().float().bfloat16().double() for e in enc]
+        vg = sd.vectors.double().requires_grad_(True)
+        ve = sd.vectors.double().requires_grad_(True)
+        sv_g, sv_e = lerp(vg, c), lerp(ve, c)
+        out_g = sum(enc[k] * sv_g[VECTOR_OF_GRID[k]] for k in range(4))
+        out_e = sum(saved[k] * sv_e[VECTOR_OF_GRID[k]] for k in range(4))
+        (((out_g + out_e) * d_out[sel].double()).sum()).backward()
+        ref_tables.append([t.grad.reshape(-1) if t.grad is not None else torch.zeros(t.numel(), dtype=torch.float64) for t in tabs])
+        ref_vec_gather.append(vg.grad if vg.grad is not None else torch.zeros_like(vg))
+        ref_vec_egrid.append(ve.grad if ve.grad is not None else torch.zeros_like(ve))
+    return ref_tables, {"gather": ref_vec_gather, "egrid": ref_vec_egrid}, enc_all
+
+
+def _saved_features(enc_all, g, cuda):
+    """Saved per-(level, grid) features [16 * 4][stride] bf16x2, each sample at a shuffled column of a wider buffer."""
+    n = enc_all.shape[0]
+    stride = n + 37
+    perm = torch.randperm(stride, generator=g)[:n]
+    bits = _bf16_bits(enc_all)                                                 # [n, 4, 32]
+    packed = bits[..., 0::2] | (bits[..., 1::2] << np.uint32(16))             # [n, 4 grids, 16 levels]
+    egrid = np.zeros((64, stride), np.uint32)
+    egrid[:, perm.numpy()] = packed.transpose(2, 1, 0).reshape(64, n)
+    return stride, {"egrid": torch.from_numpy(egrid.view(np.int32)).to(cuda), "feat_index": perm.to(torch.int32).to(cuda)}
+
+
+def _scatter(case, monkeypatch, gen, mode, schedule):
+    """The kernel's gradients for one HRF_SCATTER generation, feature source and schedule of (grid_first, grid_count)."""
+    monkeypatch.setenv("HRF_SCATTER", gen)
+    nat = case["nat"]
+    grads, sg_dev = _segment_grads(case["m"])
+    eg, fi, stride = (case["dev"]["egrid"].data_ptr(), case["dev"]["feat_index"].data_ptr(), case["stride"]) if mode == "egrid" else (None, None, 0)
+    for first, count in schedule:
+        L.check(L.lib().hrf_field_backward_tables(C.byref(nat.field), C.byref(case["samples"]), sg_dev.data_ptr(), eg, fi, stride,
+                                                  case["ws"].data_ptr(), first, count, L.stream()))
+    torch.cuda.synchronize()
+    return [g.cpu() for g in grads]
+
+
+@pytest.fixture(scope="module")
+def ragged(cuda):
+    om, m, nat, frames = _bf16_model((6, 6), cuda)
     b = synthetic_rays(96, 48, frames, ragged=True, seed=21)   # consecutive samples of a ray: neighbouring cells at the fine levels
     pos, fr = positions_of(b), b["frames"][b["ri"]]
     n = pos.shape[0]
@@ -63,52 +154,82 @@ def test_table_scatter_matches_float64_autograd(cuda, monkeypatch, staged, carry
     g = torch.Generator().manual_seed(2)
     d_out = torch.randn(n, 32, generator=g)
     d_out[::7] = 0                                            # zero upstream gradients are skipped, not scattered
-
-    # ---- reference: float64 autograd
-    ref_tables, ref_vectors = [], []
-    for s, sd in enumerate(om.segments):
-        sel = torch.from_numpy(np.nonzero(seg == s)[0])
-        tabs = [t.double().requires_grad_(True) for t in sd.grids]
-        vec = sd.vectors.double().requires_grad_(True)
-        c = xyzt[sel]
-        sv = OF.lerp_vectors(vec, c)                            # fp32 tap arithmetic (exact: vec_res is a power of two), float64 blend
-        out = sum(hashgrid.encode(tabs[k], c[:, GRID_AXES[k]], sd.log2T) * sv[VECTOR_OF_GRID[k]] for k in range(4))
-        (out * d_out[sel].double()).sum().backward()
-        ref_tables.append([t.grad.reshape(-1) for t in tabs])
-        ref_vectors.append(vec.grad)
-
-    # ---- kernel: workspace = d(features) level-major [16][n] float2 | (x,y,z,t) [n] float4 | segment [n] u8
-    ws = torch.zeros(n * 40, dtype=torch.float32, device=cuda)
-    ws[: 32 * n] = d_out.reshape(n, 16, 2).permute(1, 0, 2).reshape(-1).to(cuda)
-    ws[32 * n: 36 * n] = xyzt.reshape(-1).to(cuda)
-    ws.view(torch.uint8)[144 * n: 145 * n] = torch.from_numpy(seg.astype(np.uint8)).to(cuda)
-    grads = [torch.zeros_like(p) for p in m.hot_parameters()]
-    sg = (L.SegmentGrads * m.num_segments)()
-    for s in range(m.num_segments):
-        for k in range(4):
-            sg[s].grid[k] = grads[5 * s + k].data_ptr()
-        sg[s].vectors = grads[5 * s + 4].data_ptr()
-    scratch = [torch.zeros_like(grads[5 * s + 4]).reshape(-1) for s in range(m.num_segments)] if vec_t else []
-    for s, t_ in enumerate(scratch):
-        sg[s].vectors_t = t_.data_ptr()
-    sg_dev = torch.from_numpy(np.frombuffer(bytes(sg), dtype=np.uint8).copy()).to(cuda)
+    # fp32 tap arithmetic (exact: vec_res is a power of two), float64 blend
+    ref_tables, ref_vec, enc_all = _reference(om, seg, xyzt, d_out, OF.lerp_vectors)
+    stride, dev = _saved_features(enc_all, g, cuda)
     samples = nat.samples_query(pos.to(cuda).contiguous(), None, fr.to(cuda).to(torch.int32).contiguous())
-    for first, count in ((0, 1), (1, 3)):                      # split launches (per-table schedule)
-        L.check(L.lib().hrf_field_backward_tables(C.byref(nat.field), C.byref(samples), sg_dev.data_ptr(), None, None, 0, ws.data_ptr(),
-                                                  first, count, L.stream()))
-    for s, t_ in enumerate(scratch):
-        assert float(grads[5 * s + 4].abs().max()) == 0.0 and float(t_.abs().max()) > 0.0   # nothing went to `vectors` directly
-        L.check(L.lib().hrf_fold_vector_grads(t_.data_ptr(), grads[5 * s + 4].data_ptr(), grads[5 * s + 4].shape[1], L.stream()))
-        assert float(t_.abs().max()) == 0.0                                                   # scratch left zeroed
-    torch.cuda.synchronize()
-    for s in range(m.num_segments):
+    return dict(m=m, nat=nat, samples=samples, ws=_workspace(d_out, xyzt, seg, cuda), stride=stride, dev=dev,
+                ref_tables=ref_tables, ref_vec=ref_vec)
+
+
+SCHEDULES = {"split": ((0, 1), (1, 3)), "one": ((0, 4),), "four": ((0, 1), (1, 1), (2, 1), (3, 1)), "pairs": ((0, 2), (2, 2))}
+RAGGED = [(gen, mode, sched) for gen in ("5", "6") for mode in ("gather", "egrid") for sched in SCHEDULES]
+
+
+@pytest.mark.parametrize("gen,mode,sched", RAGGED, ids=[f"v{g_}-{'regather' if m_ == 'gather' else 'egrid+feat_index'}-{s_}" for g_, m_, s_ in RAGGED])
+def test_table_scatter_matches_float64_autograd(ragged, monkeypatch, gen, mode, sched):
+    """Ragged rays over two temporal segments of 6 frames, for both generations, both feature sources (the re-gather of
+    the bf16 tables; the saved per-grid features read through a survivor index) and several splits of the 4 grids over
+    launches (the per-table schedules)."""
+    grads = _scatter(ragged, monkeypatch, gen, mode, SCHEDULES[sched])
+    for s in range(len(ragged["ref_tables"])):
         for k in range(4):
-            got, ref = grads[5 * s + k].cpu(), ref_tables[s][k]
-            assert ((got != 0) & (ref == 0)).sum() == 0
+            got, ref = grads[5 * s + k], ragged["ref_tables"][s][k]
+            assert ((got != 0) & (ref == 0)).sum() == 0, "gradient written to an untouched table entry"
             e = _relnorm(got, ref)
             worst = float((got.double() - ref).abs().max() / ref.abs().max())
-            print(f"staged={staged} carry={carry} chunk={chunk} seg{s} grid{k}: relnorm {e:.2e} worst entry {worst:.2e} touched {(ref != 0).sum().item()}")
+            print(f"v{gen} {mode} {sched} seg{s} grid{k}: relnorm {e:.2e} worst entry {worst:.2e} touched {(ref != 0).sum().item()}")
             assert e < 1e-5 and worst < 1e-5
-        e = _relnorm(grads[5 * s + 4].cpu(), ref_vectors[s])
-        print(f"seg{s} vectors: relnorm {e:.2e}")
+        e = _relnorm(grads[5 * s + 4], ragged["ref_vec"][mode][s])
+        print(f"v{gen} {mode} {sched} seg{s} vectors: relnorm {e:.2e}")
         assert e < 1e-5
+
+
+@pytest.fixture(scope="module", params=list(CONFIGS), ids=list(CONFIGS))
+def case(request, cuda):
+    segs = CONFIGS[request.param]
+    om, m, nat, frames = _bf16_model(segs, cuda)
+    b = synthetic_rays(72, 96, frames, ragged=True, seed=31)
+    pos, fr = positions_of(b), b["frames"][b["ri"]]
+    # samples outside the dense levels' grids (x beyond 1 or below 0 after the +0.5): the kernels' cold path
+    g = torch.Generator().manual_seed(4)
+    pick = torch.randint(0, pos.shape[0], (96,), generator=g)
+    out_pos = pos[pick].clone()
+    out_pos[:48, 0] = 0.5 + 0.005 + 0.03 * torch.rand(48, generator=g)
+    out_pos[48:, 0] = -0.5 - 0.02 - 0.03 * torch.rand(48, generator=g)
+    pos, fr = torch.cat((pos, out_pos)), torch.cat((fr, fr[pick]))
+    if pos.shape[0] % 1024 == 0:
+        pos, fr = pos[:-1], fr[:-1]
+    n = pos.shape[0]
+    assert n > 2048 and n % 1024 != 0
+    seg = om.f2s[fr.numpy()]
+    if len(segs) > 1:
+        assert len(np.unique(seg)) > 1
+    xyzt = torch.cat((pos + 0.5, torch.from_numpy(om.f2t[fr.numpy()]).unsqueeze(1)), dim=1).float()
+    d_out = torch.randn(n, 32, generator=g)
+    d_out[::7] = 0                                            # zero upstream gradients are skipped, not scattered
+    ref_tables, ref_vec, enc_all = _reference(om, seg, xyzt, d_out, _lerp_vectors)   # (coordinates outside [0, 1] here)
+    stride, dev = _saved_features(enc_all, g, cuda)
+    samples = nat.samples_query(pos.to(cuda).contiguous(), None, fr.to(cuda).to(torch.int32).contiguous())
+    return dict(m=m, nat=nat, samples=samples, ws=_workspace(d_out, xyzt, seg, cuda), stride=stride, dev=dev,
+                ref_tables=ref_tables, ref_vec=ref_vec)
+
+
+@pytest.mark.parametrize("launches", ["one", "four"], ids=["grid_count4", "4x_grid_count1"])
+@pytest.mark.parametrize("mode", ["egrid", "gather"], ids=["egrid+feat_index", "regather"])
+def test_scatter_v6_matches_float64_autograd_and_v5(cuda, monkeypatch, case, mode, launches):
+    got6 = _scatter(case, monkeypatch, "6", mode, SCHEDULES["one" if launches == "one" else "four"])
+    got5 = _scatter(case, monkeypatch, "5", mode, SCHEDULES["one"])
+    for s in range(len(case["ref_tables"])):
+        for k in range(4):
+            g6, g5, ref = got6[5 * s + k], got5[5 * s + k], case["ref_tables"][s][k]
+            assert ((g6 != 0) & (ref == 0)).sum() == 0, "gradient written to an untouched table entry"
+            e = _relnorm(g6, ref)
+            worst = float((g6.double() - ref).abs().max() / ref.abs().max().clamp_min(1e-30))
+            e5 = _relnorm(g6, g5)
+            print(f"{mode} {launches} seg{s} grid{k}: relnorm {e:.2e} worst entry {worst:.2e} vs v5 {e5:.2e} touched {(ref != 0).sum().item()}")
+            assert e < 1e-5 and worst < 1e-5 and e5 < 1e-5
+        ev = _relnorm(got6[5 * s + 4], case["ref_vec"][mode][s])
+        ev5 = _relnorm(got6[5 * s + 4], got5[5 * s + 4])
+        print(f"{mode} {launches} seg{s} vectors: relnorm {ev:.2e} vs v5 {ev5:.2e}")
+        assert ev < 1e-5 and ev5 < 1e-5
