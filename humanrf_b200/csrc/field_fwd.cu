@@ -268,6 +268,7 @@ static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t s
   else if (a.comp.ray_offsets != nullptr && a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true, true>);
   else if (a.comp.ray_offsets != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, false, true>);
   else if (a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true>);
+  else if (mlp_impl != 0 && a.egrid != nullptr) rc = launch(field_forward_kernel<true, 4, true>);   // simt debug path, e_k too
   else if (mlp_impl != 0) rc = launch(field_forward_kernel<true, 4>);
   else if (a.egrid != nullptr && unroll == 2) rc = launch(field_forward_kernel<false, 5, true, 2>);
   else if (a.egrid != nullptr && unroll == 1) rc = launch(field_forward_kernel<false, 5, true, 1>);

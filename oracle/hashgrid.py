@@ -11,6 +11,8 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from .sampler import fma32
+
 PRIME_Y = np.uint32(2654435761)
 PRIME_Z = np.uint32(805459861)
 
@@ -49,8 +51,9 @@ def level_table(log2_hashmap_size: int, n_levels: int = 16, base_resolution: int
 
 
 def _fma32(a: np.ndarray, b: np.ndarray, c) -> np.ndarray:
-    """float32 fused multiply-add (product exact in float64; one extra rounding is negligible)."""
-    return (a.astype(np.float64) * b.astype(np.float64) + np.float64(c)).astype(np.float32)
+    """float32 fused multiply-add, rounded once (a float64 sum rounded again to float32 would round twice when it lands
+    on an fp32 midpoint, and that moves the cell of a position whose scale * x + 0.5 sits next to an integer)."""
+    return fma32(a, b, np.float32(c))
 
 
 def corner_indices_and_weights(x: np.ndarray, scale: np.float32, res: int, size: int, hashed: bool):

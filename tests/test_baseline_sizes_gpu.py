@@ -89,11 +89,18 @@ def test_forward_matches_oracle(cuda, pair, impl):
     scale = np.abs(ofeat).reshape(n, 16, 2).max(axis=(0, 2))
     print("per-level feature err / scale:", np.round(ferr / scale, 4))
     assert (ferr <= 2.0 ** -7 * scale + 1e-6).all(), (ferr, scale)
-    # per-(level, grid) interpolated features saved for the backward scatter: egrid[(4 l + k) * n + i]
-    eg = saved[n * 32:].view(torch.int32).view(64, n)
+    # per-(level, grid) interpolated features saved for the backward scatter: egrid[(4 l + k) * n + i].  Checked from a
+    # second run of the same path into a sentinel-filled buffer, so that nothing the kernel was asked to write can pass
+    # as the leftovers of an earlier allocation (`saved` is torch.empty); both runs must write the same bytes.
+    seg_of = om.f2s[fr.numpy()]
+    sent = torch.full((n * 160,), -1, dtype=torch.int16, device=cuda)
+    L.check(L.lib().hrf_field_forward(C.byref(nat.field), C.byref(s), 1, impl, torch.empty_like(sig).data_ptr(), None, None,
+                                      sent.data_ptr(), sent.data_ptr() + 64 * n, L.stream()))
+    torch.cuda.synchronize()
+    assert torch.equal(sent, saved.view(torch.int16))
+    eg = sent[n * 32:].view(torch.int32).view(64, n)
     lo = (eg << 16).view(torch.float32).cpu().numpy()
     hi = (eg & -65536).view(torch.float32).cpu().numpy()
-    seg_of = om.f2s[fr.numpy()]
     xyzt = torch.cat((pos + 0.5, torch.from_numpy(om.f2t[fr.numpy()]).unsqueeze(1)), dim=1).float()
     for si, sd in enumerate(om.segments):
         sel = np.nonzero(seg_of == si)[0]
