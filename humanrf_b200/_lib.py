@@ -99,7 +99,9 @@ _SIGNATURES = {
     "hrf_field_backward": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp]),
     "hrf_field_backward_mlp": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "hrf_field_backward_tables": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, i64, vp, C.c_int, C.c_int, vp]),
+    "hrf_field_backward_mlp_dirs": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "hrf_field_position_grad": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp]),
+    "hrf_ray_gradients": (C.c_int, [vp, vp, vp, vp, vp, i64, vp, vp, vp, vp]),
     "hrf_train_loss": (C.c_int, [vp, vp, vp, vp, i64, f32, f32, vp, vp, vp, vp, vp]),
     "hrf_adam_multi": (C.c_int, [vp, C.c_int, i64, f32, f32, f32, f32, f32, C.c_int, vp]),
     "hrf_peer_alloc": (C.c_int, [i64, C.POINTER(vp)]),

@@ -12,6 +12,7 @@
 //      a second, high-occupancy kernel (scatter_v6.cu, walking each cell's corners in lane pairs, scatter_pairs.cuh)
 //      issues red.global.add.v2.f32 into the fp32 table and vector-row gradients.  scatter_v5.cu, the same walk over
 //      a different CTA shape, is its reference in the tests.  (One fused kernel was latency-bound at its low occupancy.)
+// The kDirs instantiation also writes d(view directions): dCin columns 0..15 contracted with the SH Jacobian (sh4_vjp).
 #include <cstddef>
 #include <cstdlib>
 
@@ -45,6 +46,9 @@ struct BwdArgs {
   float2* dfeat;  // [16][N] float2 workspace: d(composed features)
   float4* pos4;   // [N] normalised (x,y,z,t) of every sample, for the scatter
   uint8_t* seg8;  // [N] segment index (255 = no segment)
+  // [N,3] d(view directions), written by the kDirs instantiation only.  Kept last: the offsets of the members above
+  // are the kernel-parameter offsets field_backward_kernel was compiled against.
+  float* d_dirs;
 };
 
 // D[128,Nin] = G[128,Kout] * W[Kout,Nin]  : A = gradient tile (K-major), B = forward blob read MN-major
@@ -110,8 +114,29 @@ __device__ __forceinline__ void flush_cols(float* dst, const float* acc) {
   for (int q = 0; q < 8; ++q) atomicAdd(dst + frag_col(q) * 64 + frag_row(0, q), acc[q]);
 }
 
-// kLevelUnroll: levels unrolled in the re-encode loop (only taken when the forward's features were not saved)
-template <int kLevelUnroll = 4>
+// Vector-Jacobian product of sh4 (field_common.cuh): g = sum_j dsh[j] * dSH_j/d(x, y, z), at the fp32 x, y, z sh4 evaluates.
+// The map d -> ((d + 1) * 0.5) * 2 - 1 in front of it and the bf16 rounding of the SH values behind it count as the
+// identity, as autograd treats them (tcnn's SH input gradient, x2, composed with the reference's (d + 1) * 0.5, x0.5).
+__device__ __forceinline__ void sh4_vjp(float dx, float dy, float dz, const float* dsh, float* g) {
+  const float x = ((dx + 1.f) * 0.5f) * 2.f - 1.f, y = ((dy + 1.f) * 0.5f) * 2.f - 1.f,
+              z = ((dz + 1.f) * 0.5f) * 2.f - 1.f;
+  const float xy = x * y, xz = x * z, yz = y * z, x2 = x * x, y2 = y * y, z2 = z * z;
+  constexpr float a = 0.48860251190291987f, b = 1.0925484305920792f, c = 0.94617469575755997f,
+                  e = 0.54627421529603959f, f = 0.59004358992664352f, gg = 2.8906114426405538f,
+                  h = 0.45704579946446572f, k = 0.3731763325901154f, m = 1.4453057213202769f;
+  // SH 1..15 of sh4 and their partial derivatives (SH 0 is a constant)
+  g[0] = -a * dsh[3] + b * y * dsh[4] - b * z * dsh[7] + 2.f * e * x * dsh[8] - 6.f * f * xy * dsh[9] +
+         gg * yz * dsh[10] + h * (1.f - 5.f * z2) * dsh[13] + 2.f * m * xz * dsh[14] + 3.f * f * (y2 - x2) * dsh[15];
+  g[1] = -a * dsh[1] + b * x * dsh[4] - b * z * dsh[5] - 2.f * e * y * dsh[8] + 3.f * f * (y2 - x2) * dsh[9] +
+         gg * xz * dsh[10] + h * (1.f - 5.f * z2) * dsh[11] - 2.f * m * yz * dsh[14] + 6.f * f * xy * dsh[15];
+  g[2] = a * dsh[2] - b * y * dsh[5] + 2.f * c * z * dsh[6] - b * x * dsh[7] + gg * xy * dsh[10] -
+         10.f * h * yz * dsh[11] + k * (15.f * z2 - 3.f) * dsh[12] - 10.f * h * xz * dsh[13] + m * (x2 - y2) * dsh[14];
+}
+
+// kLevelUnroll: levels unrolled in the re-encode loop (only taken when the forward's features were not saved).
+// kDirs: also write d(view directions) [N,3] to args.d_dirs (hrf_field_backward_mlp_dirs).  The kDirs = false
+// instantiations compile to the instruction stream they had before kDirs existed.
+template <int kLevelUnroll = 4, bool kDirs = false>
 __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_constant__ BwdArgs args) {
   extern __shared__ unsigned char smem_raw[];
   BwdSmem& sm = *reinterpret_cast<BwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -258,7 +283,21 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
       float dc[48];
       if (K1 == 48) frag_stage<48, 32, 16>(reinterpret_cast<float*>(sm.h2), d);
       else frag_stage<32, 32, 16>(reinterpret_cast<float*>(sm.h2), d);
+      if constexpr (kDirs) {  // columns 0..15 (SH of the view direction) in h1, whose last reader was the round just ended
+        if (K1 == 48) frag_stage<48, 16, 0>(reinterpret_cast<float*>(sm.h1), d);
+        else frag_stage<32, 16, 0>(reinterpret_cast<float*>(sm.h1), d);
+      }
       __syncthreads();
+      if constexpr (kDirs) {
+        // d(direction) = dSH^T . dCin[0..15], finished before columns 16..47 are read so that the two sets of 16 and 32
+        // values are never live together; 0 for samples without a segment and without a colour gradient
+        stage_read_row<16>(reinterpret_cast<const float*>(sm.h1), dc);
+        if (valid) {
+          float g[3] = {0.f, 0.f, 0.f};
+          if (s.seg != nullptr && args.d_rgb != nullptr) sh4_vjp(vw.dx, vw.dy, vw.dz, dc, g);
+          args.d_dirs[3 * i] = g[0], args.d_dirs[3 * i + 1] = g[1], args.d_dirs[3 * i + 2] = g[2];
+        }
+      }
       stage_read_row<32>(reinterpret_cast<const float*>(sm.h2), dc + 16);
       if (args.d_emb != nullptr && vw.cam >= 0) {  // d(camera embedding): colour-input features 31..30+E
         const int E = f.camera_embedding_dim;
@@ -328,9 +367,9 @@ __global__ void __launch_bounds__(kTile, 2) field_backward_kernel(const __grid_c
 
 using namespace hrf;
 
-extern "C" int hrf_field_backward_mlp(const hrf_field* f, const hrf_samples* s, const float* d_sigma, const float* d_rgb,
-                                      const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
-                                      float* d_camera_embeddings, void* workspace, void* stream) {
+static int field_backward_mlp(const hrf_field* f, const hrf_samples* s, const float* d_sigma, const float* d_rgb,
+                              const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
+                              float* d_camera_embeddings, float* d_directions, void* workspace, void* stream) {
   HRF_REQUIRE(f != nullptr && s != nullptr, "null argument");
   HRF_REQUIRE(f->num_segments < 255, "at most 254 temporal segments");
   if (s->num_samples == 0) return 0;
@@ -354,21 +393,45 @@ extern "C" int hrf_field_backward_mlp(const hrf_field* f, const hrf_samples* s, 
   a.dfeat = reinterpret_cast<float2*>(workspace);
   a.pos4 = reinterpret_cast<float4*>(reinterpret_cast<char*>(workspace) + 128 * (size_t)s->num_samples);
   a.seg8 = reinterpret_cast<uint8_t*>(reinterpret_cast<char*>(workspace) + 144 * (size_t)s->num_samples);
+  a.d_dirs = d_directions;
   const int64_t tiles = (s->num_samples + kTile - 1) / kTile;
   const int smem = (int)sizeof(BwdSmem) + 1024;
   const int64_t max_ctas = (int64_t)sm_count() * 2;
   const int grid = (int)(tiles < max_ctas ? tiles : max_ctas);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (d_directions != nullptr) {
+    HRF_CUDA(cudaFuncSetAttribute(field_backward_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    field_backward_kernel<4, true><<<grid, kTile, smem, st>>>(a);
+    HRF_CHECK_LAUNCH();
+    return 0;
+  }
   // HRF_BWD_UNROLL=1: experiment for round 2 (the forward gained 19 % from the smaller loop; this kernel is 155 KB of SASS)
   static const bool compact = [] { const char* e = getenv("HRF_BWD_UNROLL"); return e && e[0] == '1'; }();
   if (compact) {
     HRF_CUDA(cudaFuncSetAttribute(field_backward_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    field_backward_kernel<1><<<grid, kTile, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+    field_backward_kernel<1><<<grid, kTile, smem, st>>>(a);
   } else {
     HRF_CUDA(cudaFuncSetAttribute(field_backward_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    field_backward_kernel<4><<<grid, kTile, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+    field_backward_kernel<4><<<grid, kTile, smem, st>>>(a);
   }
   HRF_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" int hrf_field_backward_mlp(const hrf_field* f, const hrf_samples* s, const float* d_sigma, const float* d_rgb,
+                                      const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
+                                      float* d_camera_embeddings, void* workspace, void* stream) {
+  return field_backward_mlp(f, s, d_sigma, d_rgb, d_geo, feat_bf16, feat_index, d_mlp, d_camera_embeddings, nullptr,
+                            workspace, stream);
+}
+
+extern "C" int hrf_field_backward_mlp_dirs(const hrf_field* f, const hrf_samples* s, const float* d_sigma, const float* d_rgb,
+                                           const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
+                                           float* d_camera_embeddings, float* d_directions, void* workspace, void* stream) {
+  HRF_REQUIRE(s != nullptr, "null argument");
+  HRF_REQUIRE(s->num_samples == 0 || d_directions != nullptr, "null d_directions");
+  return field_backward_mlp(f, s, d_sigma, d_rgb, d_geo, feat_bf16, feat_index, d_mlp, d_camera_embeddings, d_directions,
+                            workspace, stream);
 }
 
 int hrf_launch_scatter_v5(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads, const void* grid_feat_bf16,

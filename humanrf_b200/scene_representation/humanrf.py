@@ -119,8 +119,8 @@ class HumanRF(torch.nn.Module):
     def density(self, query_input: QueryInput) -> QueryOutput:
         """sigma and the geometry features.  When ``query_input.positions`` requires grad, the backward also returns
         d(positions) [N,3] (hrf_field_position_grad): the exact derivative of what the kernels compute, grid and vector
-        terms both, with the bf16 rounding of the composed features treated as the identity.  Not covered: gradients of
-        the directions, first-order only (``create_graph=True`` is not supported)."""
+        terms both, with the bf16 rounding of the composed features treated as the identity.  First-order only
+        (``create_graph=True`` is not supported)."""
         needs_grad = self._needs_grad(query_input.positions)
         active = (self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers)
                   if self._needs_grad() else None)
@@ -131,8 +131,9 @@ class HumanRF(torch.nn.Module):
     def forward(self, query_input: QueryInput) -> QueryOutput:
         # humanrf.py:194-204: the camera embedding is looked up while training and is all zeros otherwise
         cams = query_input.camera_numbers if (self.camera_embedding_dim > 0 and query_input.is_training) else None
-        # d(positions) as in density(); the radiance reaches the positions through the geometry features
-        needs_grad = self._needs_grad(query_input.positions)
+        # d(positions) as in density(); the radiance reaches the positions through the geometry features.  d(directions)
+        # when they require grad: the SH encoding's input gradient (hrf_field_backward_mlp_dirs)
+        needs_grad = self._needs_grad(query_input.positions, query_input.directions)
         active = (self.active_segment_list(query_input.frame_numbers, query_input.unique_frame_numbers)
                   if self._needs_grad() else None)
         sigma, geo, rgb = _FieldFunction.apply(self, 1, query_input.positions, query_input.directions,
@@ -150,12 +151,12 @@ class HumanRF(torch.nn.Module):
         src = unique_frame_numbers if unique_frame_numbers is not None else frame_numbers
         return active_segments(self.frame_numbers_to_segment_numbers, src, self.num_segments).cpu().tolist()
 
-    def _needs_grad(self, positions: Optional[torch.Tensor] = None) -> bool:
-        # ctx.needs_input_grad ignores torch.no_grad(); decide outside whether to save the backward buffers.  Positions
-        # that require grad count too: their gradient needs the same saved features.
+    def _needs_grad(self, *inputs: Optional[torch.Tensor]) -> bool:
+        # ctx.needs_input_grad ignores torch.no_grad(); decide outside whether to save the backward buffers.  Inputs
+        # (positions, directions, rays) that require grad count too: their gradients need the same saved features.
         if not torch.is_grad_enabled():
             return False
-        return (positions is not None and positions.requires_grad) or any(p.requires_grad for p in self.hot_parameters())
+        return any(t is not None and t.requires_grad for t in inputs) or any(p.requires_grad for p in self.hot_parameters())
 
     def get_params(self, lr):
         params = [
@@ -399,11 +400,14 @@ class _NativeField:
         return sigma if save == "none" else (sigma, saved)
 
     def backward(self, samples: L.Samples, d_sigma, d_rgb, feat, grad_tensors: List[torch.Tensor], per_table: bool = False,
-                 d_geo=None, feat_index=None, d_positions: Optional[torch.Tensor] = None):
+                 d_geo=None, feat_index=None, d_positions: Optional[torch.Tensor] = None,
+                 d_directions: Optional[torch.Tensor] = None):
         """grad_tensors: fp32 buffers in hot_parameters() order (accumulated into).  per_table launches the scatter once
         per grid instead of once for all four.  d_geo: fp32 [N,15] gradient of the geometry features, or None.
         d_positions: fp32 [N,3] written with the position gradient (hrf_field_position_grad, after the scatter, on the
-        same workspace: the parameter gradients are the launches without it), or None."""
+        same workspace: the parameter gradients are the launches without it), or None.  d_directions: fp32 [N,3] written
+        with the view-direction gradient: the MLP backward is then hrf_field_backward_mlp_dirs, whose weight gradients and
+        workspace are hrf_field_backward_mlp's, followed by the same scatter; or None."""
         m = self.model
         dev = self._device()
         sg = (L.SegmentGrads * m.num_segments)()
@@ -421,7 +425,15 @@ class _NativeField:
         n = int(samples.num_samples)
         # `feat` with a row index = composed features of a pruning pass (no per-grid features: the scatter re-gathers)
         egrid = feat.data_ptr() + 64 * n if (feat is not None and feat_index is None and feat.numel() >= n * 160 and n > 0) else None
-        if per_table:
+        if d_directions is not None:
+            L.check(L.lib().hrf_field_backward_mlp_dirs(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb),
+                                                        L.ptr(d_geo), L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(),
+                                                        L.ptr(d_emb), d_directions.data_ptr(), ws.data_ptr(), L.stream()))
+            for k in (range(4) if per_table else (None,)):
+                L.check(L.lib().hrf_field_backward_tables(C.byref(self.field), C.byref(samples), sg_dev.data_ptr(), egrid,
+                                                          L.ptr(feat_index), 0, ws.data_ptr(), 0 if k is None else k,
+                                                          4 if k is None else 1, L.stream()))
+        elif per_table:
             L.check(L.lib().hrf_field_backward_mlp(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb),
                                                    L.ptr(d_geo), L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(), L.ptr(d_emb),
                                                    ws.data_ptr(), L.stream()))
@@ -444,18 +456,32 @@ class _NativeField:
         """The position gradient alone, for frozen parameters: the MLP backward (its weight gradients go to a scratch
         buffer that is dropped) and hrf_field_position_grad on its workspace; no table scatter.  Returns d_positions
         fp32 [N,3] (rows past a device-side live count are left as they were: zeros when allocated here)."""
+        if d_positions is None:
+            d_positions = torch.zeros((int(samples.num_samples), 3), dtype=torch.float32, device=self._device())
+        self.input_backward(samples, d_sigma, d_rgb, feat, d_geo=d_geo, feat_index=feat_index, d_positions=d_positions)
+        return d_positions
+
+    def input_backward(self, samples: L.Samples, d_sigma, d_rgb, feat, d_geo=None, feat_index=None,
+                       d_positions: Optional[torch.Tensor] = None, d_directions: Optional[torch.Tensor] = None) -> None:
+        """Gradients of the inputs alone, for frozen parameters: the MLP backward (hrf_field_backward_mlp_dirs when
+        `d_directions` is given; its weight gradients go to a scratch buffer that is dropped), then, when `d_positions`
+        is given, hrf_field_position_grad on its workspace.  No table scatter.  Both outputs are fp32 [N,3], written."""
         dev = self._device()
         n = int(samples.num_samples)
         d_mlp = torch.empty(self.model.mlp_grad_elems, dtype=torch.float32, device=dev)
         ws = torch.empty(n * 40, dtype=torch.float32, device=dev)   # 160 B / sample
-        if d_positions is None:
-            d_positions = torch.zeros((n, 3), dtype=torch.float32, device=dev)
         lib = L.lib()
-        L.check(lib.hrf_field_backward_mlp(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb), L.ptr(d_geo),
-                                           L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(), None, ws.data_ptr(), L.stream()))
-        L.check(lib.hrf_field_position_grad(C.byref(self.field), C.byref(samples), ws.data_ptr(), d_positions.data_ptr(),
-                                            L.stream()))
-        return d_positions
+        if d_directions is not None:
+            L.check(lib.hrf_field_backward_mlp_dirs(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb),
+                                                    L.ptr(d_geo), L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(), None,
+                                                    d_directions.data_ptr(), ws.data_ptr(), L.stream()))
+        else:
+            L.check(lib.hrf_field_backward_mlp(C.byref(self.field), C.byref(samples), L.ptr(d_sigma), L.ptr(d_rgb),
+                                               L.ptr(d_geo), L.ptr(feat), L.ptr(feat_index), d_mlp.data_ptr(), None,
+                                               ws.data_ptr(), L.stream()))
+        if d_positions is not None:
+            L.check(lib.hrf_field_position_grad(C.byref(self.field), C.byref(samples), ws.data_ptr(), d_positions.data_ptr(),
+                                                L.stream()))
 
 
 def _as_f32c(t: torch.Tensor) -> torch.Tensor:
@@ -485,6 +511,8 @@ class _FieldFunction(torch.autograd.Function):
                               cams if cams is not None else frames)
         ctx.has_dirs, ctx.has_cams = dirs is not None, cams is not None
         ctx.pos_dtype, ctx.pos_shape = positions.dtype, positions.shape
+        if directions is not None:
+            ctx.dir_dtype, ctx.dir_shape = directions.dtype, directions.shape
         geo_out = geo[:, 1:]            # differentiable: humanrf.py:185-186 hands sigma_net's outputs 1..15 to the caller
         if rgb is None:
             rgb = sigma.new_zeros((0, 3))
@@ -504,20 +532,29 @@ class _FieldFunction(torch.autograd.Function):
             ds = torch.zeros(pos.shape[0], dtype=torch.float32, device=pos.device)
         dg = None if d_geo is None else _as_f32c(d_geo)
         want_pos = ctx.needs_input_grad[2]
+        want_dir = ctx.needs_input_grad[3] and ctx.has_dirs and ctx.mode == 1
         d_pos = torch.empty((pos.shape[0], 3), dtype=torch.float32, device=pos.device) if want_pos else None
+        # 0 without a colour gradient: the density does not depend on the direction
+        d_dir = (torch.empty if dr is not None else torch.zeros)((pos.shape[0], 3), dtype=torch.float32,
+                                                                  device=pos.device) if want_dir else None
         if not any(ctx.needs_input_grad[8:]):
-            if not want_pos:
+            if not want_pos and not want_dir:
                 return (None,) * (8 + len(params))
             # every parameter frozen: the MLP backward and the position kernel only, no table scatter
-            nat.position_backward(samples, ds, dr, feat, d_geo=dg, d_positions=d_pos)
-            d_pos_out = d_pos.to(ctx.pos_dtype).reshape(ctx.pos_shape)
-            return (None, None, d_pos_out, None, None, None, None, None, *([None] * len(params)))
+            if want_pos or dr is not None:
+                nat.input_backward(samples, ds, dr, feat, d_geo=dg, d_positions=d_pos,
+                                   d_directions=d_dir if dr is not None else None)
+            d_pos_out = None if d_pos is None else d_pos.to(ctx.pos_dtype).reshape(ctx.pos_shape)
+            d_dir_out = None if d_dir is None else d_dir.to(ctx.dir_dtype).reshape(ctx.dir_shape)
+            return (None, None, d_pos_out, d_dir_out, None, None, None, None, *([None] * len(params)))
         grads = [torch.zeros_like(p) for p in params]
-        keep = nat.backward(samples, ds, dr, feat, grads, d_geo=dg, d_positions=d_pos)
+        keep = nat.backward(samples, ds, dr, feat, grads, d_geo=dg, d_positions=d_pos,
+                            d_directions=d_dir if dr is not None else None)
         del keep
         if ctx.active is not None:      # segments the batch did not touch get no gradient at all (None), as in the reference
             from ..parallel import mask_inactive_segment_grads
 
             grads = mask_inactive_segment_grads(grads, ctx.active)
         d_pos_out = None if d_pos is None else d_pos.to(ctx.pos_dtype).reshape(ctx.pos_shape)
-        return (None, None, d_pos_out, None, None, None, None, None, *grads)
+        d_dir_out = None if d_dir is None else d_dir.to(ctx.dir_dtype).reshape(ctx.dir_shape)
+        return (None, None, d_pos_out, d_dir_out, None, None, None, None, *grads)

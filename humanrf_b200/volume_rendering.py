@@ -12,6 +12,11 @@ returns None) and ``render`` with the reference signatures.  Differences by desi
   sigma / rgb never reach HBM;
 * ``prune_samples`` keeps the composed features of the candidates it encoded (64 B/sample) on the batch object; a
   following ``render`` of the same (unchanged) batch runs the two MLPs on them instead of encoding the survivors again.
+
+``render`` differentiates with respect to ``ray_origins``, ``ray_directions``, ``sample_distances`` and a tensor
+``background_rgb`` when they require grad, as the reference's torch-built positions and tcnn encodings do: the MLP
+backward also writes the view-direction gradient (hrf_field_backward_mlp_dirs), hrf_field_position_grad the position
+gradient, and hrf_ray_gradients reduces both per ray.  The choice of samples (sampler, prune) is not differentiated.
 """
 from __future__ import annotations
 
@@ -45,11 +50,14 @@ class RenderOutput:
         return out
 
 
-def _ray_arrays(ib: InputBatch):
-    o = L.require_cuda(ib.ray_origins.detach().float().contiguous(), "ray_origins")
-    d = L.require_cuda(ib.ray_directions.detach().float().contiguous(), "ray_directions")
+def _ray_arrays(ib: InputBatch, keep_grad: bool = False):
+    """The batch's arrays as the kernels read them.  With `keep_grad`, origins, directions and distances that require
+    grad stay attached to their graph (the conversions are then differentiable views or copies)."""
+    att = lambda x: x if (keep_grad and x.requires_grad) else x.detach()      # noqa: E731
+    o = L.require_cuda(att(ib.ray_origins).float().contiguous(), "ray_origins")
+    d = L.require_cuda(att(ib.ray_directions).float().contiguous(), "ray_directions")
     fr = L.require_cuda(ib.frame_numbers.detach().reshape(-1).to(torch.int32).contiguous(), "frame_numbers")
-    t = L.require_cuda(ib.sample_distances.detach().reshape(-1).float().contiguous(), "sample_distances")
+    t = L.require_cuda(att(ib.sample_distances).reshape(-1).float().contiguous(), "sample_distances")
     ri = L.require_cuda(ib.ray_indices.detach().reshape(-1).to(torch.int64).contiguous(), "ray_indices")
     return o, d, fr, t, ri
 
@@ -114,7 +122,8 @@ def _reusable_features(ib: InputBatch, model: HumanRF):
 
 
 class _RenderFunction(torch.autograd.Function):
-    """field forward (ray-batch form) + compositing; backward = composite bwd + fused field bwd."""
+    """field forward (ray-batch form) + compositing; backward = composite bwd + fused field bwd, then, for the ray inputs
+    that require grad, the position kernel and the per-ray reduction (hrf_ray_gradients)."""
 
     @staticmethod
     def forward(ctx, model: HumanRF, o, d, fr, t, ri, num_rays, background, step, cams, needs_grad, active, reuse, *params):
@@ -136,15 +145,18 @@ class _RenderFunction(torch.autograd.Function):
                                               L.stream()))
         ctx.model, ctx.num_rays, ctx.step, ctx.active = model, num_rays, float(step), active
         ctx.bg = bg
+        ctx.bg_shape = background.shape if isinstance(background, torch.Tensor) else None
+        ctx.bg_dtype = background.dtype if isinstance(background, torch.Tensor) else None
         ctx.save_for_backward(o, d, fr, t, ri, sigma, rgb, off, feat if feat is not None else t,
-                              cams if cams is not None else fr, src if src is not None else fr)
+                              cams if cams is not None else fr, src if src is not None else fr,
+                              wsum if ctx.needs_input_grad[7] else t)
         ctx.has_cams, ctx.has_src = cams is not None, src is not None
         return color, wsum
 
     @staticmethod
     def backward(ctx, d_color, d_wsum):
         model = ctx.model
-        o, d, fr, t, ri, sigma, rgb, off, feat, cams, src = ctx.saved_tensors
+        o, d, fr, t, ri, sigma, rgb, off, feat, cams, src, wsum = ctx.saved_tensors
         nat = model.native()
         dev = t.device
         n = t.shape[0]
@@ -156,19 +168,43 @@ class _RenderFunction(torch.autograd.Function):
                                                ctx.num_rays, ctx.step, L.ptr(ctx.bg), dc.data_ptr(), L.ptr(dw),
                                                d_sigma.data_ptr(), d_rgb.data_ptr(), L.stream()))
         params = model.hot_parameters()
-        grads = [torch.zeros_like(p) for p in params]
-        nat.backward(nat.samples_rays(o, d, fr, t, ri, cams if ctx.has_cams else None), d_sigma, d_rgb, feat, grads,
-                     feat_index=src if ctx.has_src else None)
-        if ctx.active is not None:      # segments the batch did not touch get no gradient at all (None), as in the reference
-            from .parallel import mask_inactive_segment_grads
+        samples = nat.samples_rays(o, d, fr, t, ri, cams if ctx.has_cams else None)
+        want_o, want_d, want_t, want_bg = (ctx.needs_input_grad[i] for i in (1, 2, 4, 7))
+        rays = want_o or want_d or want_t
+        d_pos = torch.empty((n, 3), dtype=torch.float32, device=dev) if rays else None
+        d_dir = torch.empty((n, 3), dtype=torch.float32, device=dev) if want_d else None
+        grads = [None] * len(params)
+        if any(ctx.needs_input_grad[13:]):
+            grads = [torch.zeros_like(p) for p in params]
+            nat.backward(samples, d_sigma, d_rgb, feat, grads, feat_index=src if ctx.has_src else None, d_positions=d_pos,
+                         d_directions=d_dir)
+            if ctx.active is not None:  # segments the batch did not touch get no gradient at all (None), as in the reference
+                from .parallel import mask_inactive_segment_grads
 
-            grads = mask_inactive_segment_grads(grads, ctx.active)
-        return (None,) * 13 + tuple(grads)
+                grads = mask_inactive_segment_grads(grads, ctx.active)
+        elif rays:                      # every parameter frozen: no table scatter
+            nat.input_backward(samples, d_sigma, d_rgb, feat, feat_index=src if ctx.has_src else None, d_positions=d_pos,
+                               d_directions=d_dir)
+        g_o = g_d = g_t = g_bg = None
+        if rays:
+            g_o = torch.empty((ctx.num_rays, 3), dtype=torch.float32, device=dev)
+            g_d = torch.empty((ctx.num_rays, 3), dtype=torch.float32, device=dev)
+            g_t = torch.empty(n, dtype=torch.float32, device=dev) if want_t else None
+            L.check(L.lib().hrf_ray_gradients(d_pos.data_ptr(), L.ptr(d_dir), t.data_ptr(), d.data_ptr(), off.data_ptr(),
+                                              ctx.num_rays, g_o.data_ptr(), g_d.data_ptr(), L.ptr(g_t), L.stream()))
+            g_o, g_d = (g_o if want_o else None), (g_d if want_d else None)
+        if want_bg:                     # color = sum w rgb + background (1 - sum w)
+            g_bg = (dc * (1.0 - wsum)).sum_to_size(ctx.bg_shape).to(ctx.bg_dtype)
+        return (None, g_o, g_d, None, g_t, None, None, g_bg) + (None,) * 5 + tuple(grads)
 
 
 def render(input_batch: InputBatch, scene_representation: HumanRF, background_rgb: torch.Tensor, is_training: bool,
            render_step_size: float = 4e-4) -> RenderOutput:
-    """volume_rendering.py:87-150.  color = sum w*rgb + background*(1 - sum w); weights_sum = sum w."""
+    """volume_rendering.py:87-150.  color = sum w*rgb + background*(1 - sum w); weights_sum = sum w.
+    Gradients reach the parameters and, when they require grad, ray_origins, ray_directions, sample_distances and a
+    tensor background_rgb.  A background that requires grad alone (frozen model, constant rays) also takes the autograd
+    route: its gradient needs only d_color and weights_sum, but the forward then saves the features and the backward
+    runs the compositing backward, which this case does not use."""
     ib = input_batch
     o, d, fr, t, ri = _ray_arrays(ib)
     cams = None
@@ -176,7 +212,11 @@ def render(input_batch: InputBatch, scene_representation: HumanRF, background_rg
         cams = L.require_cuda(ib.camera_numbers.detach().reshape(-1).to(torch.int32).contiguous(), "camera_numbers")
     params = scene_representation.hot_parameters()
     # (ctx.needs_input_grad ignores torch.no_grad(): decide here whether the backward buffers are worth saving)
-    needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
+    ray_inputs = (ib.ray_origins, ib.ray_directions, ib.sample_distances,
+                  background_rgb if isinstance(background_rgb, torch.Tensor) else None)
+    needs_grad = scene_representation._needs_grad(*ray_inputs)
+    if needs_grad and any(x is not None and x.requires_grad for x in ray_inputs[:3]):
+        o, d, _, t, _ = _ray_arrays(ib, keep_grad=True)
     reuse = _reusable_features(ib, scene_representation)
     if not needs_grad:
         color, wsum = render_fused(scene_representation, o, d, fr, t, ri, ib.num_rays, background_rgb, render_step_size, cams,

@@ -260,6 +260,15 @@ int hrf_field_backward_mlp(const hrf_field* f, const hrf_samples* s, const float
 int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* s, const hrf_segment_grads* seg_grads,
                               const void* grid_feat_bf16, const int32_t* feat_index, int64_t grid_feat_stride,
                               const void* workspace, int grid_first, int grid_count, void* stream);
+/* hrf_field_backward_mlp that also writes the view-direction gradient d_directions [N,3] (row i: sample i's direction,
+ * in the ray-batch form its ray's direction): d_dir = sum_j dCin[j] * dSH_j/d(x, y, z) over the 16 SH inputs of the colour
+ * net, at the fp32 x, y, z the forward's SH evaluates.  The map d -> ((d + 1) / 2) * 2 - 1 and the bf16 rounding of the
+ * SH values count as the identity (tcnn's SH input gradient composed with the reference's (d + 1) / 2).  Written, not
+ * accumulated, for i < live count; rows past it are untouched; rows of samples without a segment, and every row when
+ * d_rgb is NULL, are 0.  Everything else (d_mlp, d_camera_embeddings, the workspace) is as hrf_field_backward_mlp's. */
+int hrf_field_backward_mlp_dirs(const hrf_field* f, const hrf_samples* s, const float* d_sigma, const float* d_rgb,
+                                const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
+                                float* d_camera_embeddings, float* d_directions /* [N,3] */, void* workspace, void* stream);
 /* Position gradient: d_positions[i] = sum over levels l and grids k of J_{k,l}(p_i)^T . dF_l(i), the derivative of the
  * composed features hrf_field_forward computes, contracted with d(composed features).  `workspace` is what
  * hrf_field_backward_mlp filled for the same `s`: dF as float2 [16][N] at 0, normalised positions at 128 N, segment ids
@@ -271,6 +280,17 @@ int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* s, const hr
  * atomics: two runs write identical bytes.  Nothing here synchronises. */
 int hrf_field_position_grad(const hrf_field* f, const hrf_samples* s, const void* workspace,
                             float* d_positions /* [N,3] */, void* stream);
+/* Ray-form reduction of the per-sample gradients, for positions p_i = o_r + t_i d_r and view direction d_r of the
+ * samples i of ray r (ray_offsets [R+1] as hrf_ray_offsets writes it):
+ *   d_origins[r] = sum_i dpos_i;   d_ray_directions[r] = sum_i (t_i dpos_i + ddir_i);   d_sample_distances[i] = dpos_i . d_r
+ * d_directions (per-sample view-direction gradient) and d_sample_distances may be NULL.  All outputs are written, not
+ * accumulated; a ray without samples gets zeros.  A batch without samples passes d_positions = sample_distances = NULL
+ * (ray_offsets and ray_directions may then be NULL too): every ray gets zeros.  One warp per ray, a fixed summation
+ * order and no atomics: two runs write identical bytes. */
+int hrf_ray_gradients(const float* d_positions /* [N,3] */, const float* d_directions /* [N,3] or NULL */,
+                      const float* sample_distances /* [N] */, const float* ray_directions /* [R,3] */,
+                      const int32_t* ray_offsets /* [R+1] */, int64_t num_rays, float* d_origins /* [R,3] */,
+                      float* d_ray_directions /* [R,3] */, float* d_sample_distances /* [N] or NULL */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Training loss on the per-ray outputs, forward and backward in one launch (trainer.py:205-215,229-238,
