@@ -59,6 +59,13 @@ class LpipsWeights(C.Structure):
     _fields_ = [("packed", vp), ("bias", vp * 5), ("lin", vp * 5)]
 
 
+class CameraPoses(C.Structure):
+    _fields_ = [("omega", vp), ("tau", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("step", vp), ("fixed", vp),
+                ("base_inverse_krs", vp), ("base_camera_origins", vp), ("inverse_krs", vp), ("camera_origins", vp),
+                ("slot_inverse_krs", vp), ("slot_camera_origins", vp), ("slot_camera_numbers", vp), ("num_cameras", i32),
+                ("num_slots", i32)]
+
+
 ADAM_BLOCK_ELEMS = 4096
 DP_MAX_WORLD = 8
 
@@ -102,6 +109,10 @@ _SIGNATURES = {
     "hrf_field_backward_mlp_dirs": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "hrf_field_position_grad": (C.c_int, [C.POINTER(Field), C.POINTER(Samples), vp, vp, vp]),
     "hrf_ray_gradients": (C.c_int, [vp, vp, vp, vp, vp, i64, vp, vp, vp, vp]),
+    "hrf_camera_pose_grad_workspace_bytes": (i64, [C.c_int]),
+    "hrf_camera_pose_grad": (C.c_int, [vp, vp, vp, vp, i64, vp, C.c_int, vp, vp, vp, vp, vp]),
+    "hrf_camera_pose_step": (C.c_int, [C.POINTER(CameraPoses), vp, vp, vp, C.c_double, C.c_double, C.c_double,
+                                       C.c_double, vp]),
     "hrf_train_loss": (C.c_int, [vp, vp, vp, vp, i64, f32, f32, vp, vp, vp, vp, vp]),
     "hrf_adam_multi": (C.c_int, [vp, C.c_int, i64, f32, f32, f32, f32, f32, C.c_int, vp]),
     "hrf_peer_alloc": (C.c_int, [i64, C.POINTER(vp)]),

@@ -1,4 +1,5 @@
-"""Camera pose refinement against a trained, frozen model.
+"""Camera pose refinement: one camera against a trained, frozen model (``refine_camera``), and every training camera
+jointly with the field inside the fused train step (``CameraPoses``).
 
 ``refine_camera`` adjusts the extrinsics of one camera so that the model's renders from it match that camera's images
 at the given frames.  It is built on the ray gradients of ``volume_rendering.render``: the rays are built in torch from
@@ -20,15 +21,33 @@ rotation and c the camera centre, both in the loader's normalised scene units in
 
 The result is returned in the dataset camera's own convention and world units (``rotation_axisangle`` of the
 camera-to-world rotation, ``translation`` of the camera centre), so the loader's normalisation is undone and the values
-can replace the calibration's entries.  Intrinsics, per-frame poses and several cameras at once are not refined.
+can replace the calibration's entries.  Intrinsics and per-frame poses are not refined; ``CameraPoses`` refines
+several cameras at once.
+
+``CameraPoses`` gives every camera of a loader the same increment (omega_c, tau_c), learnt with the field by
+``training.FusedTrainer(camera_poses=...)``.  A batch's ray r of camera c was sampled from the current tables, so
+o_r = c_c + tau_c and d_r = exp([omega_c]x) d0_r (a rotation keeps unit length: the sampler's normalisation drops out).
+With g_o, g_d the per-ray gradients of hrf_ray_gradients, the exact gradients of the stored increments are
+
+    dL/dtau_c   = sum_{r in c} g_o[r]
+    dL/domega_c = J_l(omega_c)^T sum_{r in c} (d_r x g_d[r]),
+    J_l(w) = I + (1 - cos t)/t^2 [w]x + (t - sin t)/t^3 [w]x^2,  t = |w|   (J_l(0) = I)
+
+(hrf_camera_pose_grad).  As in ``refine_camera``, the sampler's and the prune's choice of samples is not
+differentiated.  hrf_camera_pose_step then runs Adam per camera and rewrites the loader's tables on the device.
 """
 from __future__ import annotations
 
+import copy
+import csv
+import ctypes as C
 from dataclasses import dataclass, field
-from typing import List, Sequence
+from typing import Iterable, List, Optional, Sequence
 
 import numpy as np
 import torch
+
+from .. import _lib as L
 
 
 @dataclass
@@ -183,3 +202,225 @@ def refine_camera(model, loader, camera_number: int, frame_numbers: Sequence[int
     translation = (np.asarray(cam.translation, np.float64) + tau) / scale - np.asarray(loader.scene_offset, np.float64)
     return CameraRefinement(rotation_axisangle=axisangle_of(R), translation=translation, losses=losses, omega=omega,
                             tau=tau)
+
+
+CALIBRATION_COLUMNS = ("name", "w", "h", "rx", "ry", "rz", "tx", "ty", "tz", "fx", "fy", "px", "py")
+
+
+def _camera_name(cam, c: int) -> str:
+    name = getattr(cam, "name", None)
+    return str(name) if name else f"Cam{c + 1:03d}"
+
+
+def pose_gradients(d_origins: torch.Tensor, d_ray_directions: torch.Tensor, ray_directions: torch.Tensor,
+                   camera_numbers: torch.Tensor, omega: torch.Tensor):
+    """hrf_camera_pose_grad on its own: (pose_grad float32 [C,6], ray_count int32 [C]) of a ray batch, C = len(omega)
+    (float64 [C,3]).  Reads the error word back and raises ``RuntimeError`` when a camera number is outside [0, C)."""
+    R, C_ = int(ray_directions.shape[0]), int(omega.shape[0])
+    for name, t in (("d_origins", d_origins), ("d_ray_directions", d_ray_directions), ("ray_directions", ray_directions)):
+        L.require_cuda(t, name, torch.float32)
+        if tuple(t.shape) != (R, 3):
+            raise RuntimeError(f"{name} must be [{R}, 3], got {tuple(t.shape)}")
+    L.require_cuda(camera_numbers, "camera_numbers", torch.int32)
+    L.require_cuda(omega, "omega", torch.float64)
+    if camera_numbers.numel() != R or tuple(omega.shape) != (C_, 3):
+        raise RuntimeError("camera_numbers must hold one entry per ray and omega must be [C, 3]")
+    dev = omega.device
+    lib = L.lib()
+    nbytes = int(lib.hrf_camera_pose_grad_workspace_bytes(C_))
+    if nbytes < 0:
+        raise RuntimeError(f"{C_} cameras: hrf_camera_pose_grad handles 1 to 1024")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    pose_grad = torch.empty((C_, 6), dtype=torch.float32, device=dev)
+    count = torch.empty(C_, dtype=torch.int32, device=dev)
+    error = torch.zeros(1, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        L.check(lib.hrf_camera_pose_grad(L.ptr(d_origins) if R else None, L.ptr(d_ray_directions) if R else None,
+                                         L.ptr(ray_directions) if R else None, L.ptr(camera_numbers) if R else None, R,
+                                         omega.data_ptr(), C_, pose_grad.data_ptr(), count.data_ptr(), error.data_ptr(),
+                                         ws.data_ptr(), L.stream()))
+    if int(error.cpu()[0]):
+        raise RuntimeError(f"hrf_camera_pose_grad: a camera number outside [0, {C_})")
+    return pose_grad, count
+
+
+class CameraPoses:
+    """Per-camera pose increments (omega_c, tau_c) of every camera of `loader`, learnt jointly with the field by
+    ``FusedTrainer(camera_poses=...)``: R'_c = exp([omega_c]x) R_c, c'_c = c_c + tau_c in normalised scene units, the
+    convention of ``refine_camera``.  Everything lives on the device: the increments and Adam's moments (float64), one
+    Adam step counter per camera, and the base tables (the loader's ``all_inverse_krs`` / ``all_camera_origins`` when
+    this object is built, i.e. omega = tau = 0).
+
+    Each train step from `start_step` on, the step reduces its rays' gradients per camera (hrf_camera_pose_grad) and,
+    after the field's Adam, runs Adam on every camera that had rays and is not fixed, rewriting ``all_inverse_krs``,
+    ``all_camera_origins`` and the pool slots' ``inverse_krs_cuda`` / ``camera_origins_cuda`` on the device
+    (hrf_camera_pose_step), so that the loader's next batch is sampled from the refined poses.  Draw each batch after the
+    previous step has been enqueued: the gradient assumes the batch's rays come from the current tables.  The learning
+    rate decays exponentially from `lr` at `start_step` to `lr * final_lr_ratio` `max_steps` steps later.
+
+    `fixed_cameras` never move.  Moving every camera together with the scene changes no image, so the joint problem has
+    no unique solution without an anchor; by default the loader's first training camera holds the gauge.  A camera
+    number outside the loader's cameras in a batch stops every later pose update (the step checks a device-side error
+    word) and makes ``check()`` and ``state_dict()`` raise.
+
+    Not covered: intrinsics, per-frame poses, pose refinement through the autograd ``render()`` route (``refine_camera``
+    does that for one camera), and data-parallel training (exchanging pose gradients between ranks is not implemented;
+    ``FusedTrainer`` refuses the combination)."""
+
+    def __init__(self, loader, lr: float = 2e-3, final_lr_ratio: float = 1e-2, max_steps: int = 50001,
+                 start_step: int = 0, fixed_cameras: Optional[Iterable[int]] = None, betas=(0.9, 0.99),
+                 eps: float = 1e-15):
+        self.loader = loader
+        self.lr, self.final_lr_ratio, self.max_steps, self.start_step = float(lr), float(final_lr_ratio), int(max_steps), int(start_step)
+        self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
+        for name in ("all_inverse_krs", "all_camera_origins", "inverse_krs_cuda", "camera_origins_cuda", "camera_numbers_cuda"):
+            if not getattr(loader, name).is_contiguous():
+                raise RuntimeError(f"loader.{name} is not contiguous")
+        ikr, org = loader.all_inverse_krs, loader.all_camera_origins
+        n = int(ikr.shape[0])
+        if tuple(ikr.shape) != (n, 3, 3) or tuple(org.shape) != (n, 3) or ikr.dtype != torch.float32 or org.dtype != torch.float32:
+            raise RuntimeError("loader tables must be float32 all_inverse_krs [C,3,3] and all_camera_origins [C,3]")
+        if not 1 <= n <= 1024:
+            raise RuntimeError(f"{n} cameras: pose refinement handles 1 to 1024")
+        dev = ikr.device
+        self.device, self.num_cameras = dev, n
+        self.base_inverse_krs = ikr.clone()
+        self.base_camera_origins = org.clone()
+        f64 = dict(dtype=torch.float64, device=dev)
+        self.omega = torch.zeros((n, 3), **f64)
+        self.tau = torch.zeros((n, 3), **f64)
+        self.exp_avg = torch.zeros((n, 6), **f64)
+        self.exp_avg_sq = torch.zeros((n, 6), **f64)
+        self.steps = torch.zeros(n, dtype=torch.int32, device=dev)
+        if fixed_cameras is None:
+            fixed_cameras = (int(loader.camera_numbers[0]),)
+        fixed = sorted({int(c) for c in fixed_cameras})
+        if any(c < 0 or c >= n for c in fixed):
+            raise RuntimeError(f"fixed cameras {fixed} outside [0, {n})")
+        self.fixed_cameras = tuple(fixed)
+        self.fixed = torch.zeros(n, dtype=torch.uint8, device=dev)
+        self.fixed[list(fixed)] = 1
+        self.pose_grad = torch.zeros((n, 6), dtype=torch.float32, device=dev)    # the last step's, before Adam
+        self.ray_count = torch.zeros(n, dtype=torch.int32, device=dev)
+        self.error = torch.zeros(1, dtype=torch.int32, device=dev)                # sticky: bit 0, a bad camera number
+        self.workspace = torch.empty(int(L.lib().hrf_camera_pose_grad_workspace_bytes(n)), dtype=torch.uint8, device=dev)
+        p = L.CameraPoses()
+        p.omega, p.tau, p.exp_avg, p.exp_avg_sq = (t.data_ptr() for t in (self.omega, self.tau, self.exp_avg, self.exp_avg_sq))
+        p.step, p.fixed = self.steps.data_ptr(), self.fixed.data_ptr()
+        p.base_inverse_krs, p.base_camera_origins = self.base_inverse_krs.data_ptr(), self.base_camera_origins.data_ptr()
+        p.inverse_krs, p.camera_origins = ikr.data_ptr(), org.data_ptr()
+        p.slot_inverse_krs, p.slot_camera_origins = loader.inverse_krs_cuda.data_ptr(), loader.camera_origins_cuda.data_ptr()
+        p.slot_camera_numbers = loader.camera_numbers_cuda.data_ptr()
+        p.num_cameras, p.num_slots = n, int(loader.camera_numbers_cuda.numel())
+        self._desc = p
+
+    # ---------------------------------------------------------------------------------------------- train step
+    def active(self, t: int) -> bool:
+        """Whether the train step after `t` completed steps refines the poses."""
+        return t >= self.start_step
+
+    def current_lr(self, t: int) -> float:
+        """The learning rate of the pose step after `t` completed train steps."""
+        return self.lr * self.final_lr_ratio ** min(max(t - self.start_step, 0) / max(self.max_steps, 1), 1.0)
+
+    def accumulate(self, d_origins, d_ray_directions, ray_directions, cameras, num_rays: int) -> int:
+        """Enqueues hrf_camera_pose_grad into ``pose_grad`` / ``ray_count``; no host read.  Returns the launch count."""
+        L.check(L.lib().hrf_camera_pose_grad(L.ptr(d_origins), L.ptr(d_ray_directions), L.ptr(ray_directions),
+                                             L.ptr(cameras), int(num_rays), self.omega.data_ptr(), self.num_cameras,
+                                             self.pose_grad.data_ptr(), self.ray_count.data_ptr(), self.error.data_ptr(),
+                                             self.workspace.data_ptr(), L.stream()))
+        return 2 if num_rays > 0 else 1
+
+    def step(self, t: int) -> int:
+        """Enqueues hrf_camera_pose_step at the learning rate of step `t`; no host read.  Returns the launch count."""
+        b1, b2 = self.betas
+        L.check(L.lib().hrf_camera_pose_step(C.byref(self._desc), self.pose_grad.data_ptr(), self.ray_count.data_ptr(),
+                                             self.error.data_ptr(), self.current_lr(t), b1, b2, self.eps, L.stream()))
+        return 1
+
+    def check(self) -> None:
+        """Raises ``RuntimeError`` when a batch held a camera number outside the loader's cameras (reads the device)."""
+        if int(self.error.cpu()[0]):
+            raise RuntimeError(f"a train batch held a camera number outside [0, {self.num_cameras}): the poses stopped "
+                               "updating at that step")
+
+    # ---------------------------------------------------------------------------------------------- state
+    def state_dict(self) -> dict:
+        self.check()
+        return {"omega": self.omega.cpu(), "tau": self.tau.cpu(), "exp_avg": self.exp_avg.cpu(),
+                "exp_avg_sq": self.exp_avg_sq.cpu(), "steps": self.steps.cpu(), "fixed_cameras": list(self.fixed_cameras),
+                "base_inverse_krs": self.base_inverse_krs.cpu(), "base_camera_origins": self.base_camera_origins.cpu()}
+
+    def load_state_dict(self, state: dict) -> None:
+        """Restores increments, moments and step counters in place and rewrites the loader's tables from them.  The base
+        tables must be the ones this object was built from (same dataset, same normalisation)."""
+        for name in ("base_inverse_krs", "base_camera_origins"):
+            if not torch.equal(state[name].to(self.device), getattr(self, name)):
+                raise RuntimeError(f"state_dict's {name} differ from the loader's: another dataset or normalisation")
+        with torch.no_grad():
+            for name in ("omega", "tau", "exp_avg", "exp_avg_sq", "steps"):
+                getattr(self, name).copy_(state[name])
+            fixed = sorted(int(c) for c in state["fixed_cameras"])
+            self.fixed.zero_()
+            self.fixed[fixed] = 1
+            self.fixed_cameras = tuple(fixed)
+        self._write_tables(self.loader)
+
+    def tables(self):
+        """The refined sampler tables (float32 inverse_krs [C,3,3], camera_origins [C,3]), built with ``view_table``."""
+        ikr = torch.stack([view_table(self.base_inverse_krs[c], self.omega[c]) for c in range(self.num_cameras)])
+        org = (self.base_camera_origins.to(torch.float64) + self.tau).to(torch.float32)
+        return ikr.contiguous(), org.contiguous()
+
+    def _write_tables(self, loader) -> None:
+        ikr, org = self.tables()
+        with torch.no_grad():
+            loader.all_inverse_krs.copy_(ikr)
+            loader.all_camera_origins.copy_(org)
+            cams = loader.camera_numbers_cuda.long()
+            ok = cams >= 0
+            slots = torch.nonzero(ok).view(-1)
+            loader.inverse_krs_cuda[slots] = ikr[cams[slots]]
+            loader.camera_origins_cuda[slots] = org[cams[slots]]
+
+    def apply_to(self, other_loader) -> None:
+        """Writes the refined tables into another loader over the same dataset (a validation or test loader): its
+        ``all_inverse_krs``, ``all_camera_origins`` and the tables of the pool slots that hold a camera."""
+        if tuple(other_loader.all_inverse_krs.shape) != (self.num_cameras, 3, 3):
+            raise RuntimeError(f"the loader has {other_loader.all_inverse_krs.shape[0]} cameras, not {self.num_cameras}")
+        if (float(other_loader.scene_scale) != float(self.loader.scene_scale)
+                or not np.array_equal(np.asarray(other_loader.scene_offset), np.asarray(self.loader.scene_offset))):
+            raise RuntimeError("the loader normalises the scene differently: not the same dataset")
+        self._write_tables(other_loader)
+
+    # ---------------------------------------------------------------------------------------------- export
+    def refined_cameras(self) -> list:
+        """Copies of the dataset's cameras with the refined extrinsics in the dataset's convention and world units
+        (``rotation_axisangle`` of the camera-to-world rotation, ``translation`` of the centre: the loader's
+        normalisation undone, as ``refine_camera`` does).  Intrinsics are copied through."""
+        from ..dataset.cameras import rotation_from_axisangle
+
+        omega, tau = self.omega.cpu().numpy(), self.tau.cpu().numpy()
+        scale = float(self.loader.scene_scale)
+        offset = np.asarray(self.loader.scene_offset, np.float64)
+        out = []
+        for c, cam in enumerate(self.loader.cameras):      # the loader's cameras: normalised centres, omega = tau = 0
+            rc = copy.deepcopy(cam)
+            R = rotation_increment(torch.from_numpy(omega[c])).numpy() @ rotation_from_axisangle(cam.rotation_axisangle)
+            rc.rotation_axisangle = axisangle_of(R)
+            rc.translation = (np.asarray(cam.translation, np.float64) + tau[c]) / scale - offset
+            out.append(rc)
+        return out
+
+    def write_calibration_csv(self, path) -> None:
+        """The refined cameras as an ActorsHQ ``calibration.csv`` (columns name,w,h,rx,ry,rz,tx,ty,tz,fx,fy,px,py; one row
+        per camera; focal length and principal point normalised by the image size, as the dataset's)."""
+        with open(path, "w", newline="") as fh:
+            w = csv.writer(fh)
+            w.writerow(CALIBRATION_COLUMNS)
+            for c, cam in enumerate(self.refined_cameras()):
+                r, t = np.asarray(cam.rotation_axisangle, np.float64), np.asarray(cam.translation, np.float64)
+                f, p = np.asarray(cam.focal_length, np.float64), np.asarray(cam.principal_point, np.float64)
+                w.writerow([_camera_name(cam, c), int(cam.width), int(cam.height)]
+                           + [repr(float(x)) for x in (*r, *t, *f, *p)])
+

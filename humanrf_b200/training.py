@@ -23,6 +23,12 @@ Data parallel (SURVEY 8e), one process per GPU, `exchange=`:
 
 The autograd-compatible route (humanrf_b200.volume_rendering.render + torch.optim.Adam) stays available for
 running the reference's trainer.py unchanged.
+
+Camera poses (`camera_poses=`, toolbox/camera_refinement.py CameraPoses, single GPU): from the poses' start step on, the
+MLP backward also writes the view-direction gradient (hrf_field_backward_mlp_dirs), and after the table scatter the step
+runs the position gradient on the same workspace (hrf_field_position_grad), the per-ray reduction (hrf_ray_gradients),
+the per-camera reduction (hrf_camera_pose_grad) and, after the field's Adam, the per-camera Adam that rewrites the
+loader's sampler tables (hrf_camera_pose_step).  Without it, or before its start step, the step is unchanged.
 """
 from __future__ import annotations
 
@@ -56,7 +62,13 @@ class FusedTrainer:
     def __init__(self, model: HumanRF, lr: float = 1e-2, betas=(0.9, 0.99), eps: float = 1e-15, lr_decay: float = 0.5,
                  max_steps: int = 50001, bce_loss_weight: float = 1e-3, huber_delta: float = 0.01,
                  render_step_size: float = 4e-4, world_size: int = 1, process_group=None, prune: bool = True,
-                 seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False):
+                 seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False,
+                 camera_poses=None):
+        """camera_poses: a toolbox.camera_refinement.CameraPoses over the loader the batches come from; its cameras'
+        poses are refined with the field (then step() needs `cameras`).  Single GPU only: exchanging pose gradients
+        between data-parallel ranks is not implemented, so world_size > 1 with camera_poses raises ValueError."""
+        if camera_poses is not None and world_size > 1:
+            raise ValueError("camera_poses needs world_size == 1: data-parallel pose refinement is not implemented")
         if reuse not in ("none", "feat", "feat+grid"):
             raise ValueError("reuse must be 'none', 'feat' or 'feat+grid'")
         if exchange not in ("p2p", "nccl"):
@@ -65,6 +77,7 @@ class FusedTrainer:
         self.lr_decay, self.max_steps = lr_decay, max_steps
         self.bce_w, self.delta, self.step_size = bce_loss_weight, huber_delta, render_step_size
         self.world, self.pg, self.prune, self.reuse = world_size, process_group, prune, reuse
+        self.camera_poses = camera_poses
         self.exchange = exchange if world_size > 1 else "local"
         # exchange="p2p", optional: run the exchange of hash grid k (barrier + reduce/Adam/shadow kernel on a side stream)
         # while grid k+1 is still being scattered.  The exposed exchange shrinks, but four per-grid scatter launches cost
@@ -247,9 +260,18 @@ class FusedTrainer:
         """One optimisation step on a ray batch given in InputBatch layout (device tensors; `ri` int64 as in the reference's
         InputBatch.ray_indices, or int32).  Nothing in here reads
         the device back: the step is enqueued and the call returns.  Returns the number of kernels launched, or the
-        loss value when return_loss (that one read is the caller's choice)."""
+        loss value when return_loss (that one read is the caller's choice).  With camera_poses, from its start step on,
+        `cameras` (int32 [R], the camera of each ray) is required and the poses take one Adam step too."""
         lib, nat, dev = L.lib(), self.model.native(), t.device
         launches = 0
+        poses = self.camera_poses if (self.camera_poses is not None and self.camera_poses.active(self.t)) else None
+        if poses is not None:
+            if cameras is None:
+                raise ValueError("camera_poses: step() needs the camera of every ray (`cameras`, int32 [R])")
+            cameras = L.require_cuda(cameras.reshape(-1), "cameras", torch.int32)
+            if cameras.numel() != num_rays:
+                raise ValueError(f"cameras holds {cameras.numel()} entries for {num_rays} rays")
+        t_done = self.t
         marks = [] if self.profile else None
 
         def mark(name):
@@ -355,9 +377,15 @@ class FusedTrainer:
         if self.keep_grad:
             self.grad.zero_()
         ws = torch.empty(n_cap * 40, dtype=torch.float32, device=dev)   # 160 B / sample
-        L.check(lib.hrf_field_backward_mlp(C.byref(nat.field), C.byref(samples), d_sigma.data_ptr(), d_rgb.data_ptr(), None,
-                                           feat.data_ptr(), L.ptr(src), self.mlp_grad.data_ptr(), L.ptr(self.emb_grad),
-                                           ws.data_ptr(), L.stream()))
+        if poses is None:
+            L.check(lib.hrf_field_backward_mlp(C.byref(nat.field), C.byref(samples), d_sigma.data_ptr(), d_rgb.data_ptr(), None,
+                                               feat.data_ptr(), L.ptr(src), self.mlp_grad.data_ptr(), L.ptr(self.emb_grad),
+                                               ws.data_ptr(), L.stream()))
+        else:
+            d_dir = torch.empty((n_cap, 3), dtype=torch.float32, device=dev)
+            L.check(lib.hrf_field_backward_mlp_dirs(C.byref(nat.field), C.byref(samples), d_sigma.data_ptr(), d_rgb.data_ptr(),
+                                                    None, feat.data_ptr(), L.ptr(src), self.mlp_grad.data_ptr(),
+                                                    L.ptr(self.emb_grad), d_dir.data_ptr(), ws.data_ptr(), L.stream()))
         mark("backward_mlp")
         if self.overlap_exchange:
             launches += self._scatter_and_exchange_overlapped(nat, samples, egrid, src, egrid_stride, ws, mark)
@@ -368,8 +396,22 @@ class FusedTrainer:
             if bwd_events is not None:
                 bwd_events[1].record()
             mark("scatter")
+            if poses is not None:
+                # d(positions) on the workspace the scatter read, then per ray (o, d) and per camera (omega, tau)
+                d_pos = torch.empty((n_cap, 3), dtype=torch.float32, device=dev)
+                L.check(lib.hrf_field_position_grad(C.byref(nat.field), C.byref(samples), ws.data_ptr(), d_pos.data_ptr(),
+                                                    L.stream()))
+                g_o = torch.empty((num_rays, 3), dtype=torch.float32, device=dev)
+                g_d = torch.empty((num_rays, 3), dtype=torch.float32, device=dev)
+                L.check(lib.hrf_ray_gradients(d_pos.data_ptr(), d_dir.data_ptr(), t.data_ptr(), d.data_ptr(), off.data_ptr(),
+                                              num_rays, g_o.data_ptr(), g_d.data_ptr(), None, L.stream()))
+                launches += 2 + poses.accumulate(g_o, g_d, d, cameras, num_rays)
+                mark("pose_grad")
             launches += self._exchange_and_adam()
             mark("exchange+adam")
+            if poses is not None:
+                launches += poses.step(t_done)
+                mark("pose_step")
         self.last = {"samples": count[0] if count is not None else n_cap, "loss": loss[0], "marks": marks}
         if return_loss:
             return float(loss.item())

@@ -293,6 +293,51 @@ int hrf_ray_gradients(const float* d_positions /* [N,3] */, const float* d_direc
                       float* d_ray_directions /* [R,3] */, float* d_sample_distances /* [N] or NULL */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Per-camera pose refinement in the fused train step (toolbox/camera_refinement.py CameraPoses, DESIGN.md §3.14).
+ * Camera c carries an increment (omega_c, tau_c) in normalised scene units: R' = exp([omega_c]x) R, c' = c + tau_c.  Its
+ * sampler table is (exp([omega_c]x) M_c)^T with M_c = base_inverse_krs[c]^T, its origin base_camera_origins[c] + tau_c.
+ * ---------------------------------------------------------------------------------------- */
+/* Workspace of hrf_camera_pose_grad for `num_cameras` cameras (any ray count), or -1 outside [1, 1024]. */
+int64_t hrf_camera_pose_grad_workspace_bytes(int num_cameras);
+/* Pose gradients of a ray batch sampled from the current tables (o_r = c_c + tau_c, d_r = exp([omega_c]x) d0_r):
+ *   pose_grad[c] = (J_l(omega_c)^T sum_{r in c} d_r x d_ray_directions[r],  sum_{r in c} d_origins[r])
+ *   J_l(w) = I + (1 - cos t)/t^2 [w]x + (t - sin t)/t^3 [w]x^2, t = |w|
+ * and ray_count[c] = the rays of camera c.  Written for every camera (0 for a camera without rays).  The sums are fp32
+ * in an order fixed by the batch (no float atomics): two runs write identical bytes; J_l^T is applied in float64.  A
+ * camera number outside [0, num_cameras) sets bit 0 of error[0] (or'ed, the caller zeroes it) and the ray is left out.
+ * num_cameras <= 1024.  Nothing here synchronises. */
+int hrf_camera_pose_grad(const float* d_origins /* [R,3] */, const float* d_ray_directions /* [R,3] */,
+                         const float* ray_directions /* [R,3] */, const int32_t* camera_numbers /* [R] */,
+                         int64_t num_rays, const double* omega /* [C,3] */, int num_cameras,
+                         float* pose_grad /* [C,6] */, int32_t* ray_count /* [C] */, int32_t* error /* [1] */,
+                         void* workspace, void* stream);
+typedef struct {
+  double* omega;                      /* [C,3] rotation increments */
+  double* tau;                        /* [C,3] centre increments */
+  double* exp_avg;                    /* [C,6] Adam moments, (omega, tau) order */
+  double* exp_avg_sq;                 /* [C,6] */
+  int32_t* step;                      /* [C] Adam step counters */
+  const uint8_t* fixed;               /* [C] non-zero: the camera is never moved */
+  const float* base_inverse_krs;      /* [C,3,3] tables at omega = 0 (the loader's, transposed inverse KR) */
+  const float* base_camera_origins;   /* [C,3] origins at tau = 0 */
+  float* inverse_krs;                 /* [C,3,3] rewritten: the loader's all_inverse_krs */
+  float* camera_origins;              /* [C,3] rewritten: the loader's all_camera_origins */
+  float* slot_inverse_krs;            /* [B,3,3] rewritten: the pool slots' tables */
+  float* slot_camera_origins;         /* [B,3] */
+  const int32_t* slot_camera_numbers; /* [B] camera of each slot; -1 = empty slot, left untouched */
+  int num_cameras;                    /* C, 1..1024 */
+  int num_slots;                      /* B */
+} hrf_camera_poses;
+/* One launch: Adam (torch.optim.Adam's update, float64) on (omega_c, tau_c) of every camera with ray_count[c] > 0 that
+ * is not fixed, each with its own step counter and bias correction; its tables are rebuilt in float64 from the base
+ * tables and rounded once (omega = 0 gives the base table bit for bit).  Cameras without rays, and fixed cameras, keep
+ * parameters, moments, step counter and tables.  Then every slot with a camera copies that camera's tables.  When
+ * error is non-NULL and error[0] != 0 (a bad camera number in hrf_camera_pose_grad), nothing is written.  No host read. */
+int hrf_camera_pose_step(const hrf_camera_poses* poses, const float* pose_grad /* [C,6] */,
+                         const int32_t* ray_count /* [C] */, const int32_t* error /* [1] or NULL */, double lr,
+                         double beta1, double beta2, double eps, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Training loss on the per-ray outputs, forward and backward in one launch (trainer.py:205-215,229-238,
  * utils/loss.py:4-10): gt = rgb*mask + background*(1-mask); HuberLoss(delta, mean) over [R,3] +
  * bce_weight * mean(BCE(clamp(weights_sum,0,1), mask)) with eps 1e-10.  loss_out[0] += loss (caller zeroes);
