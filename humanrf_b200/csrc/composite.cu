@@ -15,6 +15,12 @@ __device__ __forceinline__ float warp_incl_sum(float v, int lane) {
   }
   return v;
 }
+// Exclusive sum from an inclusive one: the lane before's value (0 on lane 0).  Not `incl - v`: with v = +inf that is
+// inf - inf = NaN (nerfacc's running sum renders such a sample opaque), and a large v after a small prefix cancels.
+__device__ __forceinline__ float warp_excl_of(float incl, int lane) {
+  const float e = __shfl_up_sync(0xffffffffu, incl, 1);
+  return lane == 0 ? 0.f : e;
+}
 __device__ __forceinline__ float warp_incl_prod(float v, int lane) {
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
@@ -162,7 +168,7 @@ __global__ void __launch_bounds__(256) composite_fwd_kernel(const float* __restr
       sdt = sigma[i] * __fsub_rn(__fadd_rn(t, step), t);  // sigmas * (t_ends - t_starts)
     }
     const float incl = warp_incl_sum(sdt, lane);
-    const float excl = carry + (incl - sdt);
+    const float excl = carry + warp_excl_of(incl, lane);
     const float w = in ? __expf(-excl) * (1.f - __expf(-sdt)) : 0.f;
     if (in) {
       if (weights != nullptr) weights[i] = w;
@@ -211,7 +217,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const float* __restr
       g = d0 * rgb[3 * i] + d1 * rgb[3 * i + 1] + d2 * rgb[3 * i + 2] + gw;
     }
     const float incl = warp_incl_sum(sdt, lane);
-    const float excl = carry + (incl - sdt);
+    const float excl = carry + warp_excl_of(incl, lane);
     if (in) total += g * __expf(-excl) * (1.f - __expf(-sdt));
     carry += __shfl_sync(0xffffffffu, incl, 31);
   }
@@ -230,7 +236,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const float* __restr
       g = d0 * rgb[3 * i] + d1 * rgb[3 * i + 1] + d2 * rgb[3 * i + 2] + gw;
     }
     const float incl = warp_incl_sum(sdt, lane);
-    const float excl = carry + (incl - sdt);
+    const float excl = carry + warp_excl_of(incl, lane);
     const float T = __expf(-excl), ea = __expf(-sdt);
     const float w = in ? T * (1.f - ea) : 0.f;
     const float gwv = g * w;

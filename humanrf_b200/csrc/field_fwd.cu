@@ -194,8 +194,13 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
       if (lane == 0) x_first[warp] = ray;
       if (lane == 31) x_last[warp] = ray, x_tail[warp * kTail] = depth;
       __syncthreads();
-      depth += carry_in(0);
-      const float wgt = valid ? __expf(-(depth - sdt)) * (1.f - __expf(-sdt)) : 0.f;
+      // exclusive depth = the lane before's inclusive one if it holds the same ray (not depth - sdt: inf - inf = NaN)
+      const float c_in = carry_in(0);
+      const float prev = __shfl_up_sync(0xffffffffu, depth, 1);
+      const int ray_prev = __shfl_up_sync(0xffffffffu, ray, 1);
+      const float excl = (lane > 0 && ray_prev == ray) ? prev + c_in : c_in;
+      depth += c_in;
+      const float wgt = valid ? __expf(-excl) * (1.f - __expf(-sdt)) : 0.f;
       float a0 = seg_scan(wgt * c0), a1 = seg_scan(wgt * c1), a2 = seg_scan(wgt * c2), a3 = seg_scan(wgt);
       float a4 = 0.f;
       if constexpr (kDepth) a4 = seg_scan(wgt * tmid);
