@@ -66,6 +66,11 @@ class CameraPoses(C.Structure):
                 ("num_slots", i32)]
 
 
+class CameraIntrinsics(C.Structure):
+    _fields_ = [("alpha", vp), ("beta", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("base_intrinsics", vp),
+                ("base_rotations", vp), ("rotations", vp)]
+
+
 ADAM_BLOCK_ELEMS = 4096
 DP_MAX_WORLD = 8
 
@@ -113,6 +118,10 @@ _SIGNATURES = {
     "hrf_camera_pose_grad": (C.c_int, [vp, vp, vp, vp, i64, vp, C.c_int, vp, vp, vp, vp, vp]),
     "hrf_camera_pose_step": (C.c_int, [C.POINTER(CameraPoses), vp, vp, vp, C.c_double, C.c_double, C.c_double,
                                        C.c_double, vp]),
+    "hrf_camera_calib_grad_workspace_bytes": (i64, [C.c_int]),
+    "hrf_camera_calib_grad": (C.c_int, [vp, vp, vp, vp, i64, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]),
+    "hrf_camera_calib_step": (C.c_int, [C.POINTER(CameraPoses), C.POINTER(CameraIntrinsics), vp, vp, vp, vp, C.c_double,
+                                        C.c_double, C.c_double, C.c_double, C.c_double, vp]),
     "hrf_train_loss": (C.c_int, [vp, vp, vp, vp, i64, f32, f32, vp, vp, vp, vp, vp]),
     "hrf_adam_multi": (C.c_int, [vp, C.c_int, i64, f32, f32, f32, f32, f32, C.c_int, vp]),
     "hrf_peer_alloc": (C.c_int, [i64, C.POINTER(vp)]),

@@ -338,6 +338,46 @@ int hrf_camera_pose_step(const hrf_camera_poses* poses, const float* pose_grad /
                          double beta1, double beta2, double eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Per-camera intrinsics refined with the pose (CameraPoses(intrinsics=True), DESIGN.md §3.15).  Camera c also carries
+ * alpha_c = (alpha_x, alpha_y), log focal scales, and beta_c = (beta_x, beta_y), principal-point offsets in units of the
+ * base focal length.  For a pixel (px, py) with base camera coordinates u0 = K0^-1 (px, py, 1) = (x0, y0, 1):
+ *   u' = ((x0 - beta_x) e^-alpha_x, (y0 - beta_y) e^-alpha_y, 1),  v = exp([omega_c]x) R u',  d = v / |v|
+ * i.e. fx = fx0 e^alpha_x, cx = cx0 + fx0 beta_x (same for y).  The sampler table is (exp([omega_c]x) (M0 B))^T with
+ * M0 = base_inverse_krs[c]^T and B = K0 A K0^-1 =
+ *   [[e^-ax, 0, -cx0 expm1(-ax) - fx0 bx e^-ax], [0, e^-ay, -cy0 expm1(-ay) - fy0 by e^-ay], [0, 0, 1]]
+ * in float64, rounded once; alpha = beta = 0 gives hrf_camera_pose_step's table bit for bit.
+ * ---------------------------------------------------------------------------------------- */
+/* Workspace of hrf_camera_calib_grad for `num_cameras` cameras (any ray count), or -1 outside [1, 1024]. */
+int64_t hrf_camera_calib_grad_workspace_bytes(int num_cameras);
+/* hrf_camera_pose_grad's outputs (the pose columns bit-identical to it on the same inputs) and, with R'_c = rotations[c]
+ * (row-major, the camera's current camera-to-world rotation), q = R'^T d_r, h = R'^T (g_d - d_r (d_r . g_d)):
+ *   intrinsics_grad[c] = (-sum q_x h_x, -sum q_y h_y, -e^-alpha_x sum q_z h_x, -e^-alpha_y sum q_z h_y)
+ * = d(loss)/d(alpha_x, alpha_y, beta_x, beta_y).  Same sums' order, determinism, error word and camera limit as
+ * hrf_camera_pose_grad.  Nothing here synchronises. */
+int hrf_camera_calib_grad(const float* d_origins /* [R,3] */, const float* d_ray_directions /* [R,3] */,
+                          const float* ray_directions /* [R,3] */, const int32_t* camera_numbers /* [R] */,
+                          int64_t num_rays, const double* omega /* [C,3] */, const double* alpha /* [C,2] */,
+                          const float* rotations /* [C,3,3] */, int num_cameras, float* pose_grad /* [C,6] */,
+                          float* intrinsics_grad /* [C,4] */, int32_t* ray_count /* [C] */, int32_t* error /* [1] */,
+                          void* workspace, void* stream);
+typedef struct {
+  double* alpha;                      /* [C,2] log focal scales */
+  double* beta;                       /* [C,2] principal-point offsets / base focal length */
+  double* exp_avg;                    /* [C,4] Adam moments, (alpha_x, alpha_y, beta_x, beta_y) order */
+  double* exp_avg_sq;                 /* [C,4] */
+  const double* base_intrinsics;      /* [C,4] fx0, fy0, cx0, cy0 in pixels */
+  const double* base_rotations;       /* [C,3,3] R, camera-to-world, row-major */
+  float* rotations;                   /* [C,3,3] rewritten: exp([omega_c]x) R rounded once, hrf_camera_calib_grad's input */
+} hrf_camera_intrinsics;
+/* hrf_camera_pose_step with the intrinsics: the same cameras take one Adam step on (omega, tau) at lr and on
+ * (alpha, beta) at lr_intrinsics, sharing the camera's step counter; tables as above, origin and pool slots as
+ * hrf_camera_pose_step, and rotations[c] rewritten.  Nothing is written when error[0] != 0.  No host read. */
+int hrf_camera_calib_step(const hrf_camera_poses* poses, const hrf_camera_intrinsics* intrinsics,
+                          const float* pose_grad /* [C,6] */, const float* intrinsics_grad /* [C,4] */,
+                          const int32_t* ray_count /* [C] */, const int32_t* error /* [1] or NULL */, double lr,
+                          double lr_intrinsics, double beta1, double beta2, double eps, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Training loss on the per-ray outputs, forward and backward in one launch (trainer.py:205-215,229-238,
  * utils/loss.py:4-10): gt = rgb*mask + background*(1-mask); HuberLoss(delta, mean) over [R,3] +
  * bce_weight * mean(BCE(clamp(weights_sum,0,1), mask)) with eps 1e-10.  loss_out[0] += loss (caller zeroes);
