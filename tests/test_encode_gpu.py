@@ -29,7 +29,7 @@ import pytest
 import torch
 
 import encode_oracle as E
-from helpers import make_pair, synthetic_rays
+from helpers import field_without_vectors_t as _no_vectors_t, make_pair, synthetic_rays
 from humanrf_b200 import _lib as L
 
 pytestmark = pytest.mark.gpu
@@ -143,17 +143,6 @@ def _check(tag, fa, x, fr, feat, egrid, rows=None):
     assert share < 0.01, (tag, share)
     assert (enc.seg >= 0).sum() > 0.3 * x.shape[0]
     return enc
-
-
-def _no_vectors_t(nat):
-    """A copy of the field whose segment descriptors have vectors_t = NULL: the encode then reads `vectors` itself."""
-    seg = nat.seg_dev.clone()
-    size, off = C.sizeof(L.Segment), L.Segment.vectors_t.offset
-    for s in range(nat.model.num_segments):
-        seg[s * size + off: s * size + off + 8] = 0
-    f = L.Field.from_buffer_copy(nat.field)
-    f.segments = seg.data_ptr()
-    return f, seg
 
 
 # ------------------------------------------------------------------------------------------------------ tests

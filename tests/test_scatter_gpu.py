@@ -19,14 +19,12 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import make_pair, positions_of, synthetic_rays
+from helpers import make_pair, positions_of, scatter_autograd_reference as _reference, scatter_workspace as _workspace
+from helpers import segment_grads as _segment_grads, synthetic_rays
 from humanrf_b200 import _lib as L
 from oracle import field as OF
-from oracle import hashgrid
 
 pytestmark = pytest.mark.gpu
-GRID_AXES = ([0, 1, 2], [0, 1, 3], [1, 2, 3], [0, 2, 3])     # xyz, xyt, yzt, xzt (decomposition4d.py:126-129)
-VECTOR_OF_GRID = (3, 2, 0, 1)                                 # xyz*v_t, xyt*v_z, yzt*v_x, xzt*v_y (tensor_composition.cu:49-52)
 CONFIGS = {"seg50": (50,), "seg100-100-50": (100, 100, 50)}
 
 
@@ -67,55 +65,6 @@ def _bf16_model(segs, cuda):
     nat = m.native()
     nat.refresh()
     return om, m, nat, frames
-
-
-def _workspace(d_out, xyzt, seg, cuda):
-    """What hrf_field_backward_mlp leaves for the scatter: d(features) level-major [16][n] float2 | (x,y,z,t) [n] float4
-    | segment [n] u8."""
-    n = d_out.shape[0]
-    ws = torch.zeros(n * 40, dtype=torch.float32, device=cuda)
-    ws[: 32 * n] = d_out.reshape(n, 16, 2).permute(1, 0, 2).reshape(-1).to(cuda)
-    ws[32 * n: 36 * n] = xyzt.reshape(-1).to(cuda)
-    ws.view(torch.uint8)[144 * n: 145 * n] = torch.from_numpy(seg.astype(np.uint8)).to(cuda)
-    return ws
-
-
-def _segment_grads(m):
-    """Zeroed gradients of m.hot_parameters() and the device array of hrf_segment_grads that points into them."""
-    grads = [torch.zeros_like(p) for p in m.hot_parameters()]
-    sg = (L.SegmentGrads * m.num_segments)()
-    for s in range(m.num_segments):
-        for k in range(4):
-            sg[s].grid[k] = grads[5 * s + k].data_ptr()
-        sg[s].vectors = grads[5 * s + 4].data_ptr()
-    sg_dev = torch.from_numpy(np.frombuffer(bytes(sg), dtype=np.uint8).copy()).to(grads[0].device)
-    return grads, sg_dev
-
-
-def _reference(om, seg, xyzt, d_out, lerp):
-    """float64 autograd of sum_k encode_k * lerp(vector_k) against d_out, per segment.  Table gradients do not depend on
-    the features; the vector gradients of the egrid path use the saved bf16 features, those of the re-gather path the
-    exact blend of the (bf16) tables.  Also returns every sample's exact per-grid features [n, 4, 32]."""
-    ref_tables, ref_vec_gather, ref_vec_egrid = [], [], []
-    enc_all = torch.zeros(xyzt.shape[0], 4, 32, dtype=torch.float64)
-    for s, sd in enumerate(om.segments):
-        sel = torch.from_numpy(np.nonzero(seg == s)[0])
-        tabs = [t.double().requires_grad_(True) for t in sd.grids]
-        c = xyzt[sel]
-        enc = [hashgrid.encode(tabs[k], c[:, GRID_AXES[k]], sd.log2T) for k in range(4)]
-        for k in range(4):
-            enc_all[sel, k] = enc[k].detach()
-        saved = [e.detach().float().bfloat16().double() for e in enc]
-        vg = sd.vectors.double().requires_grad_(True)
-        ve = sd.vectors.double().requires_grad_(True)
-        sv_g, sv_e = lerp(vg, c), lerp(ve, c)
-        out_g = sum(enc[k] * sv_g[VECTOR_OF_GRID[k]] for k in range(4))
-        out_e = sum(saved[k] * sv_e[VECTOR_OF_GRID[k]] for k in range(4))
-        (((out_g + out_e) * d_out[sel].double()).sum()).backward()
-        ref_tables.append([t.grad.reshape(-1) if t.grad is not None else torch.zeros(t.numel(), dtype=torch.float64) for t in tabs])
-        ref_vec_gather.append(vg.grad if vg.grad is not None else torch.zeros_like(vg))
-        ref_vec_egrid.append(ve.grad if ve.grad is not None else torch.zeros_like(ve))
-    return ref_tables, {"gather": ref_vec_gather, "egrid": ref_vec_egrid}, enc_all
 
 
 def _saved_features(enc_all, g, cuda):
