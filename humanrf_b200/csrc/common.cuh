@@ -47,6 +47,29 @@ __device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u 
 __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
+// One Adam update of one element (torch.optim.Adam, no weight decay), with every rounding spelled out so that all
+// optimiser kernels and both of their paths (float4 and scalar) produce the same bits: ptxas may otherwise contract
+// the plain multiplies and adds into FMAs differently at each call site.  Replicated tensors rely on this -- every
+// data-parallel rank updates them itself, with no broadcast.
+//   g' = g * gscale ; m' = fma(b1, m, (1-b1) g') ; v' = fma(b2, v, ((1-b2) g') g')
+//   p' = fma(-lr1, m' / (sqrt(v') / bc2s + eps), p)        lr1 = lr / (1 - b1^k), bc2s = sqrt(1 - b2^k)
+// (torch: denom = sqrt(v)/sqrt(bias_correction2) + eps ; p -= lr/bias_correction1 * m/denom.)  tests/adam_oracle.py
+// bounds each of these roundings.
+__device__ __forceinline__ void adam_update(float& p, float& m, float& v, float g, float gscale, float b1, float b2,
+                                            float one_minus_b1, float one_minus_b2, float eps, float lr1, float bc2s) {
+  g = __fmul_rn(g, gscale);
+  m = __fmaf_rn(b1, m, __fmul_rn(one_minus_b1, g));
+  v = __fmaf_rn(b2, v, __fmul_rn(__fmul_rn(one_minus_b2, g), g));
+  p = __fmaf_rn(-lr1, __fdiv_rn(m, __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2s), eps)), p);
+}
+
+// element i of a `vectors` tensor [4, VR, 32] inside its transposed copy [4, 16, VR, 2] (hrf_segment.vectors_t)
+__device__ __forceinline__ int64_t vectors_t_index(int64_t i, int vr) {
+  const int c = (int)(i & 31);
+  const int64_t row = (i >> 5) % vr, axis = (i >> 5) / vr;
+  return ((axis * 16 + (c >> 1)) * vr + row) * 2 + (c & 1);
+}
+
 // ---------------------------------------------------------------------------------------
 // mbarrier + proxies
 // ---------------------------------------------------------------------------------------

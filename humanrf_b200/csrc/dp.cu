@@ -16,12 +16,6 @@
 
 namespace hrf {
 
-__device__ __forceinline__ int64_t vectors_t_index_dp(int64_t i, int vr) {   // as vectors_t_index in train.cu
-  const int c = (int)(i & 31);
-  const int64_t row = (i >> 5) % vr, axis = (i >> 5) / vr;
-  return ((axis * 16 + (c >> 1)) * vr + row) * 2 + (c & 1);
-}
-
 struct DpPeers {
   const float* grad[HRF_DP_MAX_WORLD];
   __nv_bfloat16* shadow[HRF_DP_MAX_WORLD];
@@ -47,12 +41,8 @@ __global__ void __launch_bounds__(256) dp_reduce_adam_kernel(const DpPeers P, co
   const float lr1 = lr / bc1;
   const int64_t start = t.shard_begin + (b - t.first_block) * HRF_ADAM_BLOCK_ELEMS;
   const int64_t end = start + HRF_ADAM_BLOCK_ELEMS < t.shard_end ? start + HRF_ADAM_BLOCK_ELEMS : t.shard_end;
-  auto upd = [&](float& p, float& m, float& v, float g) {
-    g *= gscale;
-    m = b1 * m + (1.f - b1) * g;
-    v = b2 * v + (1.f - b2) * g * g;
-    p = p - lr1 * (m / (sqrtf(v) / bc2s + eps));
-  };
+  const float omb1 = 1.f - b1, omb2 = 1.f - b2;
+  auto upd = [&](float& p, float& m, float& v, float g) { adam_update(p, m, v, g, gscale, b1, b2, omb1, omb2, eps, lr1, bc2s); };
   const bool vec = t.blob_perm == nullptr && ((t.grad_offset | start | (t.shadow_offset < 0 ? 0 : t.shadow_offset)) & 3) == 0 &&
                    ((end - start) & 3) == 0 &&
                    ((reinterpret_cast<uintptr_t>(t.param) | reinterpret_cast<uintptr_t>(t.exp_avg) |
@@ -80,15 +70,15 @@ __global__ void __launch_bounds__(256) dp_reduce_adam_kernel(const DpPeers P, co
         *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(t.local_shadow_bf16) + i) = q;
       }
       if (t.vectors_t != nullptr) {
-        *reinterpret_cast<float2*>(t.vectors_t + vectors_t_index_dp(i, t.vec_res)) = make_float2(p.x, p.y);
-        *reinterpret_cast<float2*>(t.vectors_t + vectors_t_index_dp(i + 2, t.vec_res)) = make_float2(p.z, p.w);
+        *reinterpret_cast<float2*>(t.vectors_t + vectors_t_index(i, t.vec_res)) = make_float2(p.x, p.y);
+        *reinterpret_cast<float2*>(t.vectors_t + vectors_t_index(i + 2, t.vec_res)) = make_float2(p.z, p.w);
       }
     }
   } else {
     for (int64_t i = start + threadIdx.x; i < end; i += 256) {
-      float s = 0.f;
+      float s = __ldcg(P.grad[0] + t.grad_offset + i);   // rank order, as the float4 path
 #pragma unroll
-      for (int r = 0; r < kWorld; ++r) s += __ldcg(P.grad[r] + t.grad_offset + i);
+      for (int r = 1; r < kWorld; ++r) s += __ldcg(P.grad[r] + t.grad_offset + i);
       float p = t.param[i], m = t.exp_avg[i], v = t.exp_avg_sq[i];
       upd(p, m, v, s);
       t.param[i] = p, t.exp_avg[i] = m, t.exp_avg_sq[i] = v;
@@ -99,7 +89,7 @@ __global__ void __launch_bounds__(256) dp_reduce_adam_kernel(const DpPeers P, co
       } else if (t.local_shadow_bf16 != nullptr) {
         reinterpret_cast<__nv_bfloat16*>(t.local_shadow_bf16)[t.blob_perm != nullptr ? (int64_t)t.blob_perm[i] : i] = q;
       }
-      if (t.vectors_t != nullptr) t.vectors_t[vectors_t_index_dp(i, t.vec_res)] = p;
+      if (t.vectors_t != nullptr) t.vectors_t[vectors_t_index(i, t.vec_res)] = p;
     }
   }
 }

@@ -32,15 +32,12 @@ __global__ void adam_kernel(float* __restrict__ p, float* __restrict__ m, float*
                             const float* __restrict__ g, __nv_bfloat16* __restrict__ shadow, int64_t n, float lr,
                             float b1, float b2, float eps, float bc1, float bc2_sqrt, float gscale) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const float lr1 = lr / bc1;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const float gi = g[i] * gscale;
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
+    float pi = p[i], mi = m[i], vi = v[i];
+    adam_update(pi, mi, vi, g[i], gscale, b1, b2, 1.f - b1, 1.f - b2, eps, lr1, bc2_sqrt);
     m[i] = mi;
     v[i] = vi;
-    // torch: denom = sqrt(v)/sqrt(bias_correction2) + eps ; p -= lr/bias_correction1 * m/denom
-    const float denom = sqrtf(vi) / bc2_sqrt + eps;
-    const float pi = p[i] - (lr / bc1) * (mi / denom);
     p[i] = pi;
     if (shadow != nullptr) shadow[i] = __float2bfloat16_rn(pi);
   }

@@ -8,13 +8,6 @@
 
 namespace hrf {
 
-// element i of a `vectors` tensor [4, VR, 32] inside its transposed copy [4, 16, VR, 2]
-__device__ __forceinline__ int64_t vectors_t_index(int64_t i, int vr) {
-  const int c = (int)(i & 31);
-  const int64_t row = (i >> 5) % vr, axis = (i >> 5) / vr;
-  return ((axis * 16 + (c >> 1)) * vr + row) * 2 + (c & 1);
-}
-
 __global__ void transpose_vectors_kernel(const float* __restrict__ v, float* __restrict__ vt, int vr) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < (int64_t)4 * vr * 32) vt[vectors_t_index(i, vr)] = v[i];
@@ -92,13 +85,8 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(const hrf_adam_tensor* 
   const int64_t start = (b - t.first_block) * HRF_ADAM_BLOCK_ELEMS;
   const int64_t end = start + HRF_ADAM_BLOCK_ELEMS < t.n ? start + HRF_ADAM_BLOCK_ELEMS : t.n;
   __nv_bfloat16* sh = reinterpret_cast<__nv_bfloat16*>(t.shadow_bf16);
-  auto upd = [&](float& p, float& m, float& v, float g) {
-    g *= gscale;
-    m = b1 * m + (1.f - b1) * g;
-    v = b2 * v + (1.f - b2) * g * g;
-    // torch: denom = sqrt(v)/sqrt(bias_correction2) + eps ; p -= lr/bias_correction1 * m/denom
-    p = p - lr1 * (m / (sqrtf(v) / bc2s + eps));
-  };
+  const float omb1 = 1.f - b1, omb2 = 1.f - b2;
+  auto upd = [&](float& p, float& m, float& v, float g) { adam_update(p, m, v, g, gscale, b1, b2, omb1, omb2, eps, lr1, bc2s); };
   const bool vec = t.blob_perm == nullptr &&
                    ((reinterpret_cast<uintptr_t>(t.param) | reinterpret_cast<uintptr_t>(t.exp_avg) |
                      reinterpret_cast<uintptr_t>(t.exp_avg_sq) | reinterpret_cast<uintptr_t>(t.grad)) & 15u) == 0 &&
