@@ -211,52 +211,60 @@ __global__ void __launch_bounds__(256) ray_minmax_kernel(const __grid_constant__
   }
 }
 
-// Single-CTA dual exclusive scan over the R candidate rays: kept-ray positions and sample offsets.
+// Single-CTA dual exclusive scan over the R candidate rays: kept-ray positions and sample offsets.  The sample sums
+// run in 64 bits, so counters[1] is the exact total even past 2^31 - 1; the per-ray offsets stay int32 (the caller
+// refuses totals they cannot hold before any sample is written).
 __global__ void __launch_bounds__(1024) ray_scan_kernel(const uint8_t* __restrict__ mask,
                                                         const int32_t* __restrict__ counts, int64_t n,
                                                         int32_t* __restrict__ ray_pos, int32_t* __restrict__ sample_pos,
                                                         int64_t* __restrict__ counters) {
-  __shared__ int2 warp_tot[32];
-  __shared__ int2 carry;
+  __shared__ int warp_m[32];
+  __shared__ long long warp_c[32];
+  __shared__ long long carry_m, carry_c;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) carry = make_int2(0, 0);
+  if (tid == 0) carry_m = 0, carry_c = 0;
   __syncthreads();
   for (int64_t base = 0; base < n; base += 1024) {
     const int64_t i = base + tid;
     const int m = (i < n) ? (int)mask[i] : 0;
-    const int c = (i < n && m) ? counts[i] : 0;
-    int sm = m, sc = c;
+    const long long c = (i < n && m) ? counts[i] : 0;
+    int sm = m;
+    long long sc = c;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
-      const int tm = __shfl_up_sync(0xffffffffu, sm, d), tc = __shfl_up_sync(0xffffffffu, sc, d);
+      const int tm = __shfl_up_sync(0xffffffffu, sm, d);
+      const long long tc = __shfl_up_sync(0xffffffffu, sc, d);
       if (lane >= d) sm += tm, sc += tc;
     }
-    if (lane == 31) warp_tot[wid] = make_int2(sm, sc);
+    if (lane == 31) warp_m[wid] = sm, warp_c[wid] = sc;
     __syncthreads();
     if (wid == 0) {
-      int2 t = warp_tot[lane];
-      int am = t.x, ac = t.y;
+      const int tm0 = warp_m[lane];
+      const long long tc0 = warp_c[lane];
+      int am = tm0;
+      long long ac = tc0;
 #pragma unroll
       for (int d = 1; d < 32; d <<= 1) {
-        const int tm = __shfl_up_sync(0xffffffffu, am, d), tc = __shfl_up_sync(0xffffffffu, ac, d);
+        const int tm = __shfl_up_sync(0xffffffffu, am, d);
+        const long long tc = __shfl_up_sync(0xffffffffu, ac, d);
         if (lane >= d) am += tm, ac += tc;
       }
-      warp_tot[lane] = make_int2(am - t.x, ac - t.y);  // exclusive warp offsets
+      warp_m[lane] = am - tm0;  // exclusive warp offsets
+      warp_c[lane] = ac - tc0;
     }
     __syncthreads();
-    const int2 wo = warp_tot[wid];
-    const int2 cr = carry;
+    const long long om = carry_m + warp_m[wid], oc = carry_c + warp_c[wid];
     if (i < n) {
-      ray_pos[i] = cr.x + wo.x + sm - m;
-      sample_pos[i] = cr.y + wo.y + sc - c;
+      ray_pos[i] = (int32_t)(om + sm - m);
+      sample_pos[i] = (int32_t)(oc + sc - c);
     }
     __syncthreads();
-    if (tid == 1023) carry = make_int2(cr.x + wo.x + sm, cr.y + wo.y + sc);
+    if (tid == 1023) carry_m = om + sm, carry_c = oc + sc;
     __syncthreads();
   }
   if (tid == 0) {
-    counters[0] = carry.x;
-    counters[1] = carry.y;
+    counters[0] = carry_m;
+    counters[1] = carry_c;
   }
 }
 

@@ -18,6 +18,8 @@ import torch
 
 from .. import _lib as L
 
+INT32_MAX = 2**31 - 1  # sample offsets and relative ray indices are int32, as in the reference's API
+
 
 def _get_data(occupancy: bool, samples: bool, rgba, light_mask, frame_numbers, camera_numbers, grid_texture_objects,
               landscape_modes, all_ray_indices, inverse_krs, camera_origins, aabb, grid_resolution, image_width,
@@ -76,6 +78,9 @@ def _get_data(occupancy: bool, samples: bool, rgba, light_mask, frame_numbers, c
                                  kept_idx.data_ptr(), offs.data_ptr(), counters.data_ptr(), ws.data_ptr(), ws_bytes,
                                  L.stream()))
     n_rays, n_samples = (int(v) for v in counters.cpu())  # the one host sync of the call
+    if n_samples > INT32_MAX:
+        raise RuntimeError(f"ray sampler: {n_samples} samples in one call exceed the int32 sample offsets' cap of "
+                           f"{INT32_MAX} (2^31 - 1); sample fewer rays per call or use a coarser raymarching step")
     o, d, mm = o[:n_rays], d[:n_rays], mm[:n_rays]
     fn, cn, kept_idx = fn[:n_rays], cn[:n_rays], kept_idx[:n_rays]
     if pool_on_gpu:

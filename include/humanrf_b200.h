@@ -55,7 +55,9 @@ int hrf_occgrid_lookup(int64_t handle, int grid_resolution, const float* points_
  *                        (optionally AND NOT light_mask, :254-257), device-side compaction,
  *                        per-ray gathers (:258-266) and per-ray sample counts/offsets
  *                        (:283-290, occupancy filter of :183-189 already applied).
- *                        counters[0]=R' (kept rays), counters[1]=N' (kept samples).
+ *                        counters[0]=R' (kept rays), counters[1]=N' (kept samples).  N' is summed
+ *                        in 64 bits and exact, but sample_offsets are int32: a caller must not
+ *                        call hrf_sampler_samples when N' > 2^31 - 1 (the offsets have wrapped).
  *   hrf_sampler_samples: compute_sample_distances_kernel (:149-194) + final compaction
  *                        (:322-323) written directly at the scanned offsets.
  * rgba_pool / light_mask are DEVICE-resident pools here (the reference indexes a CPU pool and
