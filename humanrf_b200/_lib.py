@@ -79,6 +79,10 @@ class DpPeers(C.Structure):
     _fields_ = [("grad", vp * DP_MAX_WORLD), ("shadow", vp * DP_MAX_WORLD), ("world", i32), ("rank", i32)]
 
 
+class CameraGradRecords(C.Structure):
+    _fields_ = [("record", vp * DP_MAX_WORLD), ("world", i32), ("rank", i32)]
+
+
 class DpTensor(C.Structure):
     _fields_ = [("param", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("grad_offset", i64), ("shadow_offset", i64),
                 ("local_shadow_bf16", vp), ("blob_perm", vp), ("active", vp), ("step", vp), ("n", i64),
@@ -130,6 +134,12 @@ _SIGNATURES = {
     "hrf_peer_open": (C.c_int, [vp, C.POINTER(vp)]),
     "hrf_peer_close": (C.c_int, [vp]),
     "hrf_dp_reduce_adam": (C.c_int, [C.POINTER(DpPeers), vp, C.c_int, i64, i64, C.c_int, f32, f32, f32, f32, f32, vp]),
+    "hrf_camera_grad_record_bytes": (i64, [C.c_int]),
+    "hrf_camera_pose_step_ranks": (C.c_int, [C.POINTER(CameraPoses), C.POINTER(CameraGradRecords), vp, C.c_double,
+                                             C.c_double, C.c_double, C.c_double, vp]),
+    "hrf_camera_calib_step_ranks": (C.c_int, [C.POINTER(CameraPoses), C.POINTER(CameraIntrinsics),
+                                              C.POINTER(CameraGradRecords), vp, C.c_double, C.c_double, C.c_double,
+                                              C.c_double, C.c_double, vp]),
     "hrf_compose_tensors_forward": (C.c_int, [vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_backward": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),

@@ -28,6 +28,10 @@
 //   dL/dalpha_x = -sum_r q_x h_x,   dL/dbeta_x = -e^-alpha_x sum_r q_z h_x   (same for y)
 // needs only d_r, g_d and R'_c.  The same two launches sum the four extra terms beside the pose's six: the pose columns
 // take the same lane tree and block order, so they are bit-identical to hrf_camera_pose_grad's.
+//
+// Data parallel (hrf_camera_pose_step_ranks, hrf_camera_calib_step_ranks, DESIGN.md §3.16): one single-CTA launch per rank
+// reduces the W ranks' gradient records in rank order and runs the same per-camera step (camera_step_body) and slot copy
+// as the single-rank kernels.
 #include <type_traits>
 
 #include "common.cuh"
@@ -282,92 +286,51 @@ __global__ void __launch_bounds__(128) calib_finish_kernel(const CalibSlot* __re
   pose_finish_body<true>(partials, num_blocks, num_cameras, omega, alpha, pose_grad, intrinsics_grad, ray_count);
 }
 
-__global__ void __launch_bounds__(256) pose_step_kernel(hrf_camera_poses p, const float* __restrict__ pose_grad,
-                                                        const int32_t* __restrict__ ray_count,
-                                                        const int32_t* __restrict__ error, double lr, double beta1,
-                                                        double beta2, double eps) {
-  if (error != nullptr && *error != 0) return;
-  for (int c = threadIdx.x; c < p.num_cameras; c += blockDim.x) {
-    if (ray_count[c] == 0 || p.fixed[c] != 0) continue;
-    const int step = p.step[c] + 1;
-    p.step[c] = step;
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2s = sqrt(1.0 - pow(beta2, (double)step));
-#pragma unroll
-    for (int k = 0; k < 6; ++k) {
-      const double g = (double)pose_grad[6 * c + k];
-      const double m = beta1 * p.exp_avg[6 * c + k] + (1.0 - beta1) * g;
-      const double v = beta2 * p.exp_avg_sq[6 * c + k] + (1.0 - beta2) * g * g;
-      p.exp_avg[6 * c + k] = m, p.exp_avg_sq[6 * c + k] = v;
-      double* q = k < 3 ? p.omega + 3 * c + k : p.tau + 3 * c + k - 3;
-      *q -= lr / bc1 * (m / (sqrt(v) / bc2s + eps));   // torch.optim.Adam
-    }
-    // table: (exp([w]x) M)^T with M = T^T, T the base table: T'[i][j] = sum_k R[j][k] T[i][k]
-    const double w[3] = {p.omega[3 * c], p.omega[3 * c + 1], p.omega[3 * c + 2]};
-    double a, b, cc, R[9], T[9];
-    so3_coeffs(w[0] * w[0] + w[1] * w[1] + w[2] * w[2], a, b, cc);
-    so3_matrix(w, a, b, R);
-#pragma unroll
-    for (int i = 0; i < 9; ++i) T[i] = (double)p.base_inverse_krs[9 * c + i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-      for (int j = 0; j < 3; ++j)
-        p.inverse_krs[9 * c + 3 * i + j] =
-            (float)(R[3 * j] * T[3 * i] + R[3 * j + 1] * T[3 * i + 1] + R[3 * j + 2] * T[3 * i + 2]);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) p.camera_origins[3 * c + k] = (float)((double)p.base_camera_origins[3 * c + k] + p.tau[3 * c + k]);
-  }
-  __syncthreads();                // the per-camera tables written above are visible to the whole block
-  for (int s = threadIdx.x; s < p.num_slots; s += blockDim.x) {
-    const int c = p.slot_camera_numbers[s];
-    if (c < 0 || c >= p.num_cameras) continue;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) p.slot_inverse_krs[9 * s + i] = p.inverse_krs[9 * c + i];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) p.slot_camera_origins[3 * s + k] = p.camera_origins[3 * c + k];
-  }
+// One torch.optim.Adam update of x: m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g g, x -= lr / bc1 * m / (sqrt(v) / bc2s + eps)
+// in float64, every rounding spelled out.  Left to the compiler, which products are fused into an FMA depends on the
+// kernel around the update, and every step kernel must give the same bits from the same gradient.
+__device__ __forceinline__ void adam_update(double g, double& m_io, double& v_io, double& x, double lr_bc1, double bc2s,
+                                            double beta1, double beta2, double eps) {
+  const double m = __fma_rn(m_io, beta1, __dmul_rn(1.0 - beta1, g));
+  const double v = __fma_rn(v_io, beta2, __dmul_rn(__dmul_rn(1.0 - beta2, g), g));
+  m_io = m, v_io = v;
+  x = __fma_rn(-lr_bc1, m / (sqrt(v) / bc2s + eps), x);
 }
 
-// hrf_camera_calib_step: pose_step_kernel's Adam and origin for (omega, tau), Adam at lr_intrinsics for (alpha, beta)
-// with the same step counter, then the table (exp([omega]x) M0 B)^T in float64, rounded once.  B = K0 A K0^-1 acts on
-// the base table's rows: T'0 = e^-ax T0, T'1 = e^-ay T1, T'2 = T2 + B02 T0 + B12 T1 with
-// B02 = -cx0 expm1(-ax) - fx0 bx e^-ax.  A zero B02 / B12 is not added, so alpha = beta = 0 gives M0 exactly (signed
-// zeros included) and the table equals pose_step_kernel's bit for bit.  The current rotation exp([omega]x) R is
-// rewritten for the next hrf_camera_calib_grad.
-__global__ void __launch_bounds__(256) calib_step_kernel(hrf_camera_poses p, hrf_camera_intrinsics q,
-                                                         const float* __restrict__ pose_grad,
-                                                         const float* __restrict__ intrinsics_grad,
-                                                         const int32_t* __restrict__ ray_count,
-                                                         const int32_t* __restrict__ error, double lr,
-                                                         double lr_intrinsics, double beta1, double beta2, double eps) {
-  if (error != nullptr && *error != 0) return;
-  for (int c = threadIdx.x; c < p.num_cameras; c += blockDim.x) {
-    if (ray_count[c] == 0 || p.fixed[c] != 0) continue;
-    const int step = p.step[c] + 1;
-    p.step[c] = step;
-    const double bc1 = 1.0 - pow(beta1, (double)step), bc2s = sqrt(1.0 - pow(beta2, (double)step));
+// Adam on camera c's (omega, tau) at lr and, with kCalib, on its (alpha, beta) at lr_intrinsics with the same step
+// counter; then its table and origin (and with kCalib its rotation) in float64, rounded once.  grad(k) is the camera's
+// gradient entry k in float64: 0..5 the pose, 6..9 the intrinsics.  Every step kernel runs this for a camera it moves.
+//
+// Without intrinsics the table is (exp([w]x) M)^T with M = T^T, T the base table: T'[i][j] = sum_k R[j][k] T[i][k].
+// With them it is (exp([omega]x) M0 B)^T in float64, rounded once.  B = K0 A K0^-1 acts on the base table's rows:
+// T'0 = e^-ax T0, T'1 = e^-ay T1, T'2 = T2 + B02 T0 + B12 T1 with B02 = -cx0 expm1(-ax) - fx0 bx e^-ax.  A zero B02 / B12
+// is not added, so alpha = beta = 0 gives M0 exactly (signed zeros included) and the table equals the pose-only one bit
+// for bit.  The current rotation exp([omega]x) R is rewritten for the next hrf_camera_calib_grad.
+template <bool kCalib, class Grad>
+__device__ __forceinline__ void camera_step_body(const hrf_camera_poses& p, const hrf_camera_intrinsics& q, int c,
+                                                 Grad grad, double lr, double lr_intrinsics, double beta1, double beta2,
+                                                 double eps) {
+  const int step = p.step[c] + 1;
+  p.step[c] = step;
+  const double bc1 = 1.0 - pow(beta1, (double)step), bc2s = sqrt(1.0 - pow(beta2, (double)step));
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
-      const double g = (double)pose_grad[6 * c + k];
-      const double m = beta1 * p.exp_avg[6 * c + k] + (1.0 - beta1) * g;
-      const double v = beta2 * p.exp_avg_sq[6 * c + k] + (1.0 - beta2) * g * g;
-      p.exp_avg[6 * c + k] = m, p.exp_avg_sq[6 * c + k] = v;
-      double* x = k < 3 ? p.omega + 3 * c + k : p.tau + 3 * c + k - 3;
-      *x -= lr / bc1 * (m / (sqrt(v) / bc2s + eps));     // torch.optim.Adam
-    }
+  for (int k = 0; k < 6; ++k) {
+    double* x = k < 3 ? p.omega + 3 * c + k : p.tau + 3 * c + k - 3;
+    adam_update(grad(k), p.exp_avg[6 * c + k], p.exp_avg_sq[6 * c + k], *x, lr / bc1, bc2s, beta1, beta2, eps);
+  }
+  if constexpr (kCalib) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const double g = (double)intrinsics_grad[4 * c + k];
-      const double m = beta1 * q.exp_avg[4 * c + k] + (1.0 - beta1) * g;
-      const double v = beta2 * q.exp_avg_sq[4 * c + k] + (1.0 - beta2) * g * g;
-      q.exp_avg[4 * c + k] = m, q.exp_avg_sq[4 * c + k] = v;
       double* x = k < 2 ? q.alpha + 2 * c + k : q.beta + 2 * c + k - 2;
-      *x -= lr_intrinsics / bc1 * (m / (sqrt(v) / bc2s + eps));
+      adam_update(grad(6 + k), q.exp_avg[4 * c + k], q.exp_avg_sq[4 * c + k], *x, lr_intrinsics / bc1, bc2s, beta1, beta2,
+                  eps);
     }
-    const double w[3] = {p.omega[3 * c], p.omega[3 * c + 1], p.omega[3 * c + 2]};
-    double a, b, cc, R[9], T[9];
-    so3_coeffs(w[0] * w[0] + w[1] * w[1] + w[2] * w[2], a, b, cc);
-    so3_matrix(w, a, b, R);
+  }
+  const double w[3] = {p.omega[3 * c], p.omega[3 * c + 1], p.omega[3 * c + 2]};
+  double a, b, cc, R[9], T[9];
+  so3_coeffs(w[0] * w[0] + w[1] * w[1] + w[2] * w[2], a, b, cc);
+  so3_matrix(w, a, b, R);
+  if constexpr (kCalib) {
     const double ax = q.alpha[2 * c], ay = q.alpha[2 * c + 1], bx = q.beta[2 * c], by = q.beta[2 * c + 1];
     const double fx0 = q.base_intrinsics[4 * c], fy0 = q.base_intrinsics[4 * c + 1];
     const double cx0 = q.base_intrinsics[4 * c + 2], cy0 = q.base_intrinsics[4 * c + 3];
@@ -381,14 +344,19 @@ __global__ void __launch_bounds__(256) calib_step_kernel(hrf_camera_poses p, hrf
       if (b12 != 0.0) t2 += b12 * t1;
       T[k] = t0 * ex, T[3 + k] = t1 * ey, T[6 + k] = t2;
     }
+  } else {
 #pragma unroll
-    for (int i = 0; i < 3; ++i)
+    for (int i = 0; i < 9; ++i) T[i] = (double)p.base_inverse_krs[9 * c + i];
+  }
 #pragma unroll
-      for (int j = 0; j < 3; ++j)
-        p.inverse_krs[9 * c + 3 * i + j] =
-            (float)(R[3 * j] * T[3 * i] + R[3 * j + 1] * T[3 * i + 1] + R[3 * j + 2] * T[3 * i + 2]);
+  for (int i = 0; i < 3; ++i)
 #pragma unroll
-    for (int k = 0; k < 3; ++k) p.camera_origins[3 * c + k] = (float)((double)p.base_camera_origins[3 * c + k] + p.tau[3 * c + k]);
+    for (int j = 0; j < 3; ++j)
+      p.inverse_krs[9 * c + 3 * i + j] =
+          (float)(R[3 * j] * T[3 * i] + R[3 * j + 1] * T[3 * i + 1] + R[3 * j + 2] * T[3 * i + 2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) p.camera_origins[3 * c + k] = (float)((double)p.base_camera_origins[3 * c + k] + p.tau[3 * c + k]);
+  if constexpr (kCalib) {
     const double* Rb = q.base_rotations + 9 * c;
 #pragma unroll
     for (int i = 0; i < 3; ++i)
@@ -396,7 +364,11 @@ __global__ void __launch_bounds__(256) calib_step_kernel(hrf_camera_poses p, hrf
       for (int j = 0; j < 3; ++j)
         q.rotations[9 * c + 3 * i + j] = (float)(R[3 * i] * Rb[j] + R[3 * i + 1] * Rb[3 + j] + R[3 * i + 2] * Rb[6 + j]);
   }
-  __syncthreads();                // the per-camera tables written above are visible to the whole block
+}
+
+// Every pool slot that holds a camera copies that camera's tables.  The caller has synchronised the block after the
+// per-camera tables were written.
+__device__ __forceinline__ void slot_copy_body(const hrf_camera_poses& p) {
   for (int s = threadIdx.x; s < p.num_slots; s += blockDim.x) {
     const int c = p.slot_camera_numbers[s];
     if (c < 0 || c >= p.num_cameras) continue;
@@ -405,6 +377,103 @@ __global__ void __launch_bounds__(256) calib_step_kernel(hrf_camera_poses p, hrf
 #pragma unroll
     for (int k = 0; k < 3; ++k) p.slot_camera_origins[3 * s + k] = p.camera_origins[3 * c + k];
   }
+}
+
+__global__ void __launch_bounds__(256) pose_step_kernel(hrf_camera_poses p, const float* __restrict__ pose_grad,
+                                                        const int32_t* __restrict__ ray_count,
+                                                        const int32_t* __restrict__ error, double lr, double beta1,
+                                                        double beta2, double eps) {
+  if (error != nullptr && *error != 0) return;
+  const hrf_camera_intrinsics none{};
+  for (int c = threadIdx.x; c < p.num_cameras; c += blockDim.x) {
+    if (ray_count[c] == 0 || p.fixed[c] != 0) continue;
+    camera_step_body<false>(p, none, c, [&](int k) { return (double)pose_grad[6 * c + k]; }, lr, 0.0, beta1, beta2, eps);
+  }
+  __syncthreads();                // the per-camera tables written above are visible to the whole block
+  slot_copy_body(p);
+}
+
+// hrf_camera_calib_step: pose_step_kernel's Adam and origin for (omega, tau), Adam at lr_intrinsics for (alpha, beta)
+// with the same step counter, then the table with the intrinsics and the rotation (camera_step_body<true>).
+__global__ void __launch_bounds__(256) calib_step_kernel(hrf_camera_poses p, hrf_camera_intrinsics q,
+                                                         const float* __restrict__ pose_grad,
+                                                         const float* __restrict__ intrinsics_grad,
+                                                         const int32_t* __restrict__ ray_count,
+                                                         const int32_t* __restrict__ error, double lr,
+                                                         double lr_intrinsics, double beta1, double beta2, double eps) {
+  if (error != nullptr && *error != 0) return;
+  for (int c = threadIdx.x; c < p.num_cameras; c += blockDim.x) {
+    if (ray_count[c] == 0 || p.fixed[c] != 0) continue;
+    camera_step_body<true>(p, q, c,
+                           [&](int k) { return k < 6 ? (double)pose_grad[6 * c + k] : (double)intrinsics_grad[4 * c + k - 6]; },
+                           lr, lr_intrinsics, beta1, beta2, eps);
+  }
+  __syncthreads();                // the per-camera tables written above are visible to the whole block
+  slot_copy_body(p);
+}
+
+// The data-parallel step (hrf_camera_pose_step_ranks / hrf_camera_calib_step_ranks, DESIGN.md §3.16), one CTA on every
+// rank over the same W records (header: the record layout).
+//   1. Any rank's error word set: nothing is written; a rank that sees bit 0 (a bad camera number) in ANOTHER rank's
+//      word sets bit 1 of its own sticky word.  Bit 0 is only written by the gradient kernels, which every rank's
+//      barrier orders before this kernel, so every rank takes the same decision even while a peer sets its bit 1.
+//   2. The records are staged into shared memory, one record word per thread and step, coalesced: the gradient entry
+//      as (sum over r = 0..W-1 in rank order of (double)grad_r) / W, the camera's touched flag as the OR of the ray
+//      counts.  At W = 1 the entry is (double)grad_0 exactly: the single-rank kernels' input.
+//   3. Every touched camera that is not fixed takes camera_step_body, then the slots are copied.
+constexpr int kRankStepThreads = 384;
+
+template <bool kCalib>
+__global__ void __launch_bounds__(kRankStepThreads) step_ranks_kernel(hrf_camera_poses p, hrf_camera_intrinsics q,
+                                                                      hrf_camera_grad_records rec, int32_t* error,
+                                                                      double lr, double lr_intrinsics, double beta1,
+                                                                      double beta2, double eps) {
+  extern __shared__ double sgrad[];                    // [C][10] reduced gradients, then int32 touched [C]
+  const int C = p.num_cameras, W = rec.world;
+  int any = 0, peer_bad = 0;
+#pragma unroll
+  for (int r = 0; r < HRF_DP_MAX_WORLD; ++r) {
+    if (r < W) {
+      const int e = reinterpret_cast<const int32_t*>(rec.record[r])[11 * C];
+      any |= e;
+      if (r != rec.rank) peer_bad |= e & 1;
+    }
+  }
+  if (any != 0) {
+    if (threadIdx.x == 0 && peer_bad != 0) atomicOr(error, 2);
+    return;
+  }
+  int* touched = reinterpret_cast<int*>(sgrad + 10 * C);
+  constexpr int kSums = kCalib ? 10 : 6;
+  const int n_sums = kSums * C;
+  for (int i = threadIdx.x; i < n_sums + C; i += blockDim.x) {
+    const int word = i < n_sums ? i : 10 * C + (i - n_sums);      // pose [6C] | intrinsics [4C] | ray counts [C]
+    uint32_t v[HRF_DP_MAX_WORLD];
+#pragma unroll
+    for (int r = 0; r < HRF_DP_MAX_WORLD; ++r)
+      if (r < W) v[r] = reinterpret_cast<const uint32_t*>(rec.record[r])[word];
+    if (i < n_sums) {
+      double s = (double)__uint_as_float(v[0]);
+#pragma unroll
+      for (int r = 1; r < HRF_DP_MAX_WORLD; ++r)
+        if (r < W) s += (double)__uint_as_float(v[r]);
+      const int c = i < 6 * C ? i / 6 : (i - 6 * C) / 4, k = i < 6 * C ? i % 6 : 6 + (i - 6 * C) % 4;
+      sgrad[10 * c + k] = s / (double)W;
+    } else {
+      uint32_t seen = 0;
+#pragma unroll
+      for (int r = 0; r < HRF_DP_MAX_WORLD; ++r)
+        if (r < W) seen |= v[r];
+      touched[i - n_sums] = seen != 0;
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    if (touched[c] == 0 || p.fixed[c] != 0) continue;
+    camera_step_body<kCalib>(p, q, c, [&](int k) { return sgrad[10 * c + k]; }, lr, lr_intrinsics, beta1, beta2, eps);
+  }
+  __syncthreads();                // the per-camera tables written above are visible to the whole block
+  slot_copy_body(p);
 }
 
 }  // namespace hrf
@@ -520,4 +589,57 @@ extern "C" int hrf_camera_calib_step(const hrf_camera_poses* poses, const hrf_ca
                                                                            error, lr, lr_intrinsics, beta1, beta2, eps);
   HRF_CHECK_LAUNCH();
   return 0;
+}
+
+extern "C" int64_t hrf_camera_grad_record_bytes(int num_cameras) {
+  if (num_cameras < 1 || num_cameras > kPoseMaxCameras) return -1;
+  return (int64_t)(11 * num_cameras + 1) * 4;
+}
+
+static int step_ranks(bool calib, const hrf_camera_poses* poses, const hrf_camera_intrinsics* intrinsics,
+                      const hrf_camera_grad_records* records, int32_t* error, double lr, double lr_intrinsics,
+                      double beta1, double beta2, double eps, void* stream) {
+  HRF_REQUIRE(poses != nullptr && records != nullptr && error != nullptr, "null argument");
+  const hrf_camera_poses& p = *poses;
+  const hrf_camera_grad_records& rec = *records;
+  HRF_REQUIRE(p.num_cameras >= 1 && p.num_cameras <= kPoseMaxCameras, "camera count outside [1, 1024]");
+  HRF_REQUIRE(p.num_slots >= 0, "negative slot count");
+  HRF_REQUIRE(rec.world >= 1 && rec.world <= HRF_DP_MAX_WORLD, "world size outside [1, 8]");
+  HRF_REQUIRE(rec.rank >= 0 && rec.rank < rec.world, "rank outside [0, world)");
+  for (int r = 0; r < rec.world; ++r) HRF_REQUIRE(rec.record[r] != nullptr, "null gradient record");
+  HRF_REQUIRE(p.omega && p.tau && p.exp_avg && p.exp_avg_sq && p.step && p.fixed && p.base_inverse_krs &&
+                  p.base_camera_origins && p.inverse_krs && p.camera_origins,
+              "null camera table");
+  HRF_REQUIRE(p.num_slots == 0 || (p.slot_inverse_krs && p.slot_camera_origins && p.slot_camera_numbers),
+              "null slot table");
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t smem = (size_t)p.num_cameras * (10 * sizeof(double) + sizeof(int));
+  if (calib) {
+    HRF_REQUIRE(intrinsics != nullptr, "null argument");
+    const hrf_camera_intrinsics& q = *intrinsics;
+    HRF_REQUIRE(q.alpha && q.beta && q.exp_avg && q.exp_avg_sq && q.base_intrinsics && q.base_rotations && q.rotations,
+                "null intrinsics table");
+    if (smem > 48 * 1024)     // more than 585 cameras
+      HRF_CUDA(cudaFuncSetAttribute(step_ranks_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    step_ranks_kernel<true><<<1, kRankStepThreads, smem, st>>>(p, q, rec, error, lr, lr_intrinsics, beta1, beta2, eps);
+  } else {
+    if (smem > 48 * 1024)
+      HRF_CUDA(cudaFuncSetAttribute(step_ranks_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    step_ranks_kernel<false><<<1, kRankStepThreads, smem, st>>>(p, hrf_camera_intrinsics{}, rec, error, lr, 0.0, beta1,
+                                                                beta2, eps);
+  }
+  HRF_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int hrf_camera_pose_step_ranks(const hrf_camera_poses* poses, const hrf_camera_grad_records* records,
+                                          int32_t* error, double lr, double beta1, double beta2, double eps,
+                                          void* stream) {
+  return step_ranks(false, poses, nullptr, records, error, lr, 0.0, beta1, beta2, eps, stream);
+}
+
+extern "C" int hrf_camera_calib_step_ranks(const hrf_camera_poses* poses, const hrf_camera_intrinsics* intrinsics,
+                                           const hrf_camera_grad_records* records, int32_t* error, double lr,
+                                           double lr_intrinsics, double beta1, double beta2, double eps, void* stream) {
+  return step_ranks(true, poses, intrinsics, records, error, lr, lr_intrinsics, beta1, beta2, eps, stream);
 }

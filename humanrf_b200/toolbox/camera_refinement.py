@@ -53,6 +53,7 @@ from __future__ import annotations
 import copy
 import csv
 import ctypes as C
+import hashlib
 from dataclasses import dataclass, field
 from typing import Iterable, List, Optional, Sequence
 
@@ -380,14 +381,26 @@ class CameraPoses:
     intrinsics and rotations).  `fixed_cameras` freeze the intrinsics too.  With `intrinsics=False` nothing differs
     from the pose-only refinement: the same kernels, ``state_dict`` keys and tensors.
 
-    Not covered: lens distortion, per-frame poses or intrinsics, pose refinement through the autograd ``render()`` route
-    (``refine_camera`` does that for one camera), and data-parallel training (exchanging pose gradients between ranks is
-    not implemented; ``FusedTrainer`` refuses the combination)."""
+    Data-parallel training (DESIGN.md §3.16): build one ``CameraPoses`` per rank over that rank's loader with
+    `world_size` and `process_group` set as the trainer's; the construction checks, as a collective, that every rank has
+    the same cameras, base tables, fixed cameras and settings (``ValueError`` on every rank otherwise).  Each rank's step
+    writes its gradient record (``pose_grad``, ``intrinsics_grad``, ``ray_count``, ``error``: views of ``record``); the
+    trainer lets every rank read every record, and every rank takes the same step: the gradient is the rank-ordered sum
+    over the ranks divided by `world_size`, a camera seen by any rank moves on every rank, and a bad camera number on
+    any rank stops the poses on every rank (``check()`` raises everywhere).  The replicas stay bit-identical, so
+    ``state_dict()`` of rank 0 is enough; ``load_state_dict()`` is called on every rank with the same state.
+
+    Not covered: lens distortion, per-frame poses or intrinsics, and pose refinement through the autograd ``render()``
+    route (``refine_camera`` does that for one camera)."""
 
     def __init__(self, loader, lr: float = 2e-3, final_lr_ratio: float = 1e-2, max_steps: int = 50001,
                  start_step: int = 0, fixed_cameras: Optional[Iterable[int]] = None, betas=(0.9, 0.99),
-                 eps: float = 1e-15, intrinsics: bool = False, intrinsics_lr: float = 1e-3):
+                 eps: float = 1e-15, intrinsics: bool = False, intrinsics_lr: float = 1e-3, world_size: int = 1,
+                 process_group=None):
         self.loader = loader
+        self.world_size, self.process_group = int(world_size), process_group
+        if not 1 <= self.world_size <= L.DP_MAX_WORLD:
+            raise ValueError(f"world_size {world_size} outside [1, {L.DP_MAX_WORLD}]")
         self.lr, self.final_lr_ratio, self.max_steps, self.start_step = float(lr), float(final_lr_ratio), int(max_steps), int(start_step)
         self.intrinsics, self.intrinsics_lr = bool(intrinsics), float(intrinsics_lr)
         self.betas, self.eps = (float(betas[0]), float(betas[1])), float(eps)
@@ -418,9 +431,10 @@ class CameraPoses:
         self.fixed_cameras = tuple(fixed)
         self.fixed = torch.zeros(n, dtype=torch.uint8, device=dev)
         self.fixed[list(fixed)] = 1
-        self.pose_grad = torch.zeros((n, 6), dtype=torch.float32, device=dev)    # the last step's, before Adam
-        self.ray_count = torch.zeros(n, dtype=torch.int32, device=dev)
-        self.error = torch.zeros(1, dtype=torch.int32, device=dev)                # sticky: bit 0, a bad camera number
+        # the gradient record (include/humanrf_b200.h): pose_grad, intrinsics_grad, ray_count and the error word are
+        # views of one allocation, what data-parallel ranks exchange
+        self.record = torch.zeros(int(L.lib().hrf_camera_grad_record_bytes(n)), dtype=torch.uint8, device=dev)
+        self._bind_record()
         ws_bytes = (L.lib().hrf_camera_calib_grad_workspace_bytes if self.intrinsics
                     else L.lib().hrf_camera_pose_grad_workspace_bytes)(n)
         self.workspace = torch.empty(int(ws_bytes), dtype=torch.uint8, device=dev)
@@ -435,6 +449,51 @@ class CameraPoses:
         p.slot_camera_numbers = loader.camera_numbers_cuda.data_ptr()
         p.num_cameras, p.num_slots = n, int(loader.camera_numbers_cuda.numel())
         self._desc = p
+        self.rank = 0
+        if self.world_size > 1:
+            import torch.distributed as dist
+
+            self.rank = dist.get_rank(process_group)
+            self._check_replicas_agree()
+
+    def _bind_record(self) -> None:
+        n, words = self.num_cameras, self.record.view(torch.int32)
+        self.pose_grad = words[:6 * n].view(torch.float32).view(n, 6)           # the last step's, before Adam
+        if self.intrinsics:
+            self.intrinsics_grad = words[6 * n:10 * n].view(torch.float32).view(n, 4)
+        self.ray_count = words[10 * n:11 * n]
+        self.error = words[11 * n:]     # sticky: bit 0, a bad camera number; bit 1, one in another rank's batch
+
+    def _adopt_record(self, buffer: torch.Tensor) -> None:
+        """Moves the gradient record into `buffer` (uint8, the record's size: peer-visible memory the other ranks read)."""
+        with torch.no_grad():
+            buffer.copy_(self.record)
+        self.record = buffer
+        self._bind_record()
+
+    def _replica_config(self) -> dict:
+        digest = lambda t: hashlib.sha256(t.detach().cpu().contiguous().numpy().tobytes()).hexdigest()   # noqa: E731
+        return {"num_cameras": self.num_cameras, "base_inverse_krs": digest(self.base_inverse_krs),
+                "base_camera_origins": digest(self.base_camera_origins), "fixed_cameras": self.fixed_cameras,
+                "intrinsics": self.intrinsics,
+                "base_intrinsics": digest(self.base_intrinsics) if self.intrinsics else None,
+                "lr": self.lr, "intrinsics_lr": self.intrinsics_lr, "final_lr_ratio": self.final_lr_ratio,
+                "max_steps": self.max_steps, "start_step": self.start_step, "betas": self.betas, "eps": self.eps}
+
+    def _check_replicas_agree(self) -> None:
+        """Collective over `process_group`: every rank must build the same cameras with the same settings, or their
+        replicas would step apart.  Every rank gathers every rank's configuration and takes the same decision, so either
+        all ranks go on or all raise ``ValueError`` naming the first field that differs."""
+        import torch.distributed as dist
+
+        mine = self._replica_config()
+        configs = [None] * self.world_size
+        dist.all_gather_object(configs, mine, group=self.process_group)
+        for name in mine:
+            values = [cfg[name] for cfg in configs]
+            if any(v != values[0] for v in values):
+                raise ValueError(f"CameraPoses differ between the ranks in {name}: every rank needs the same cameras "
+                                 "and settings")
 
     def _init_intrinsics(self, loader, n: int, dev) -> None:
         from ..dataset.cameras import rotation_from_axisangle
@@ -451,7 +510,6 @@ class CameraPoses:
         self.beta = torch.zeros((n, 2), **f64)
         self.intrinsics_exp_avg = torch.zeros((n, 4), **f64)
         self.intrinsics_exp_avg_sq = torch.zeros((n, 4), **f64)
-        self.intrinsics_grad = torch.zeros((n, 4), dtype=torch.float32, device=dev)   # the last step's, before Adam
         q = L.CameraIntrinsics()
         q.alpha, q.beta = self.alpha.data_ptr(), self.beta.data_ptr()
         q.exp_avg, q.exp_avg_sq = self.intrinsics_exp_avg.data_ptr(), self.intrinsics_exp_avg_sq.data_ptr()
@@ -489,10 +547,28 @@ class CameraPoses:
                                              self.workspace.data_ptr(), L.stream()))
         return 2 if num_rays > 0 else 1
 
-    def step(self, t: int) -> int:
+    def step(self, t: int, records: Optional[Sequence[int]] = None) -> int:
         """Enqueues hrf_camera_pose_step (hrf_camera_calib_step with intrinsics) at the learning rates of step `t`; no
-        host read.  Returns the launch count."""
+        host read.  Returns the launch count.  `records`: with world_size > 1, the device addresses of every rank's
+        gradient record in rank order (this rank's own or a gathered copy of it included); the step then reduces them
+        (hrf_camera_pose_step_ranks / hrf_camera_calib_step_ranks) and every rank takes the same step."""
         b1, b2 = self.betas
+        if records is not None:
+            if len(records) != self.world_size:
+                raise ValueError(f"{len(records)} gradient records for world_size {self.world_size}")
+            rec = L.CameraGradRecords()
+            for r, a in enumerate(records):
+                rec.record[r] = a
+            rec.world = self.world_size
+            rec.rank = self.rank
+            if self.intrinsics:
+                L.check(L.lib().hrf_camera_calib_step_ranks(C.byref(self._desc), C.byref(self._idesc), C.byref(rec),
+                                                            self.error.data_ptr(), self.current_lr(t),
+                                                            self.current_intrinsics_lr(t), b1, b2, self.eps, L.stream()))
+            else:
+                L.check(L.lib().hrf_camera_pose_step_ranks(C.byref(self._desc), C.byref(rec), self.error.data_ptr(),
+                                                           self.current_lr(t), b1, b2, self.eps, L.stream()))
+            return 1
         if self.intrinsics:
             L.check(L.lib().hrf_camera_calib_step(C.byref(self._desc), C.byref(self._idesc), self.pose_grad.data_ptr(),
                                                   self.intrinsics_grad.data_ptr(), self.ray_count.data_ptr(),
@@ -505,9 +581,13 @@ class CameraPoses:
 
     def check(self) -> None:
         """Raises ``RuntimeError`` when a batch held a camera number outside the loader's cameras (reads the device)."""
-        if int(self.error.cpu()[0]):
+        err = int(self.error.cpu()[0])
+        if err & 1:
             raise RuntimeError(f"a train batch held a camera number outside [0, {self.num_cameras}): the poses stopped "
                                "updating at that step")
+        if err:
+            raise RuntimeError(f"another rank's train batch held a camera number outside [0, {self.num_cameras}): the "
+                               "poses stopped updating at that step on every rank")
 
     # ---------------------------------------------------------------------------------------------- state
     _INTRINSICS_STATE = ("alpha", "beta", "intrinsics_exp_avg", "intrinsics_exp_avg_sq")

@@ -24,11 +24,14 @@ Data parallel (SURVEY 8e), one process per GPU, `exchange=`:
 The autograd-compatible route (humanrf_b200.volume_rendering.render + torch.optim.Adam) stays available for
 running the reference's trainer.py unchanged.
 
-Camera poses (`camera_poses=`, toolbox/camera_refinement.py CameraPoses, single GPU): from the poses' start step on, the
-MLP backward also writes the view-direction gradient (hrf_field_backward_mlp_dirs), and after the table scatter the step
-runs the position gradient on the same workspace (hrf_field_position_grad), the per-ray reduction (hrf_ray_gradients),
-the per-camera reduction (hrf_camera_pose_grad) and, after the field's Adam, the per-camera Adam that rewrites the
-loader's sampler tables (hrf_camera_pose_step).  Without it, or before its start step, the step is unchanged.
+Camera poses (`camera_poses=`, toolbox/camera_refinement.py CameraPoses): from the poses' start step on, the MLP backward
+also writes the view-direction gradient (hrf_field_backward_mlp_dirs), and after the table scatter the step runs the
+position gradient on the same workspace (hrf_field_position_grad), the per-ray reduction (hrf_ray_gradients), the
+per-camera reduction (hrf_camera_pose_grad) and, after the field's Adam, the per-camera Adam that rewrites the loader's
+sampler tables (hrf_camera_pose_step).  Data parallel (DESIGN.md §3.16): every rank's per-camera gradient record is read
+by every rank -- over NVLink between the exchange's two barriers ("p2p") or gathered after the bucket all-reduce
+("nccl") -- and one step kernel (hrf_camera_pose_step_ranks) reduces them in rank order, so every replica takes the same
+pose step.  Without camera_poses, or before its start step, the step is unchanged.
 """
 from __future__ import annotations
 
@@ -65,10 +68,18 @@ class FusedTrainer:
                  seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False,
                  camera_poses=None):
         """camera_poses: a toolbox.camera_refinement.CameraPoses over the loader the batches come from; its cameras'
-        poses are refined with the field (then step() needs `cameras`).  Single GPU only: exchanging pose gradients
-        between data-parallel ranks is not implemented, so world_size > 1 with camera_poses raises ValueError."""
-        if camera_poses is not None and world_size > 1:
-            raise ValueError("camera_poses needs world_size == 1: data-parallel pose refinement is not implemented")
+        poses are refined with the field (then step() needs `cameras`).  Its world_size must be this trainer's: with
+        world_size > 1 every rank builds its own CameraPoses over its own loader, the ranks exchange their per-camera
+        gradient records and every rank takes the same pose step (DESIGN.md §3.16).  overlap_exchange=True does not
+        take camera_poses with world_size > 1 (ValueError)."""
+        if camera_poses is not None:
+            if getattr(camera_poses, "world_size", None) != world_size:
+                raise ValueError(f"camera_poses was built for world_size {getattr(camera_poses, 'world_size', None)}, "
+                                 f"the trainer has world_size {world_size}")
+            if world_size > 1 and getattr(camera_poses, "process_group", None) is not process_group:
+                raise ValueError("camera_poses was built over another process_group than the trainer's")
+            if world_size > 1 and overlap_exchange:
+                raise ValueError("camera_poses with world_size > 1 needs overlap_exchange=False")
         if reuse not in ("none", "feat", "feat+grid"):
             raise ValueError("reuse must be 'none', 'feat' or 'feat+grid'")
         if exchange not in ("p2p", "nccl"):
@@ -84,6 +95,8 @@ class FusedTrainer:
         # more than one: off by default.
         self.overlap_exchange = bool(overlap_exchange) and self.exchange == "p2p"
         self.rank = dist.get_rank(process_group) if world_size > 1 else 0
+        if camera_poses is not None and camera_poses.rank != self.rank:
+            raise ValueError(f"camera_poses has rank {camera_poses.rank}, the trainer rank {self.rank}")
         self.params: List[torch.nn.Parameter] = model.hot_parameters()
         dev = self.params[0].device
         self.dev = dev
@@ -128,6 +141,8 @@ class FusedTrainer:
         if self.world > 1:
             self._bar = torch.zeros(1, dtype=torch.float32, device=dev)
             self._side = torch.cuda.Stream(dev)
+        if camera_poses is not None and self.world > 1:
+            self._adopt_pose_records(camera_poses)
 
     # ---------------------------------------------------------------------------------------------- set-up
     def _peer_buffer(self, nbytes: int) -> torch.Tensor:
@@ -171,6 +186,18 @@ class FusedTrainer:
         nat.adopt_shadows(views)
         self.peer_grad = self._exchange_handles(self.grad)
         self.peer_shadow = self._exchange_handles(self.shadow_flat)
+
+    def _adopt_pose_records(self, poses) -> None:
+        """Where every rank's pose-gradient record is read from.  p2p: the record moves into peer-visible memory and the
+        ranks' addresses are exchanged once; nccl: the records are gathered into one local [world, record] tensor."""
+        nbytes = int(poses.record.numel())
+        if self.exchange == "p2p":
+            poses._adopt_record(self._peer_buffer(nbytes))
+            self.peer_pose_record = self._exchange_handles(poses.record)
+            self.pose_records = list(self.peer_pose_record)
+        else:
+            self.pose_gather = torch.zeros((self.world, nbytes), dtype=torch.uint8, device=self.dev)
+            self.pose_records = [self.pose_gather[r].data_ptr() for r in range(self.world)]
 
     def _build_descriptors(self) -> None:
         m, nat, S = self.model, self.nat, self.model.num_segments
@@ -407,9 +434,9 @@ class FusedTrainer:
                                               num_rays, g_o.data_ptr(), g_d.data_ptr(), None, L.stream()))
                 launches += 2 + poses.accumulate(g_o, g_d, d, cameras, num_rays)
                 mark("pose_grad")
-            launches += self._exchange_and_adam()
+            launches += self._exchange_and_adam(poses if self.world > 1 else None, t_done)
             mark("exchange+adam")
-            if poses is not None:
+            if poses is not None and self.world == 1:
                 launches += poses.step(t_done)
                 mark("pose_step")
         self.last = {"samples": count[0] if count is not None else n_cap, "loss": loss[0], "marks": marks}
@@ -417,7 +444,9 @@ class FusedTrainer:
             return float(loss.item())
         return launches
 
-    def _exchange_and_adam(self) -> int:
+    def _exchange_and_adam(self, poses=None, t_done: int = 0) -> int:
+        """The field's exchange and Adam; with `poses` (world_size > 1) also the pose step, which reads every rank's
+        gradient record."""
         lib = L.lib()
         lr = self.current_lr()
         self.t += 1
@@ -428,17 +457,27 @@ class FusedTrainer:
             return 2
         if self.exchange == "nccl":
             dist.all_reduce(self.grad, group=self.pg)
+            if poses is not None:
+                dist.all_gather_into_tensor(self.pose_gather, poses.record, group=self.pg)
             L.check(lib.hrf_adam_multi(self.adam_desc.data_ptr(), len(self.params), self.adam_blocks, lr, b1, b2, self.eps,
                                        1.0 / self.world, 1, L.stream()))
+            if poses is not None:
+                return 4 + poses.step(t_done, self.pose_records)
             return 3
         # barrier A: every rank's gradients are complete
         dist.all_reduce(self._bar, group=self.pg)
         L.check(lib.hrf_dp_reduce_adam(C.byref(self.peers), self.adam_desc.data_ptr(), len(self.params), 0, self.adam_blocks, 1, lr,
                                        b1, b2, self.eps, 1.0 / self.world, L.stream()))
-        # barrier B: every peer has read this rank's bucket and written this rank's shadow slices
+        launches = 6
+        if poses is not None:
+            # Reads every rank's pose-gradient record over NVLink, so it must come before barrier B: B is what stops a
+            # fast peer from starting its next step's accumulate() (which rewrites its record) while this rank is still
+            # reading it.
+            launches += poses.step(t_done, self.pose_records)
+        # barrier B: every peer has read this rank's bucket (and pose record) and written this rank's shadow slices
         dist.all_reduce(self._bar, group=self.pg)
         self.grad.zero_()
-        return 6
+        return launches
 
     def _scatter_and_exchange_overlapped(self, nat, samples, egrid, src, egrid_stride, ws, mark) -> int:
         """exchange="p2p", overlapped: the scatter runs one hash grid per launch; as soon as grid k's launch is queued, a side
@@ -484,4 +523,6 @@ class FusedTrainer:
                 if r != self.rank:
                     lib.hrf_peer_close(self.peer_grad[r])
                     lib.hrf_peer_close(self.peer_shadow[r])
+                    if self.camera_poses is not None:
+                        lib.hrf_peer_close(self.peer_pose_record[r])
             self._peer_ptrs = []      # the buffers themselves stay alive as long as tensors view them (process lifetime)

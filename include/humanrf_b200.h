@@ -483,6 +483,33 @@ int hrf_dp_reduce_adam(const hrf_dp_peers* peers /* host */, const hrf_dp_tensor
                        float eps, float grad_scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Camera poses (and intrinsics) in data-parallel training (DESIGN.md §3.16).  Each rank's hrf_camera_pose_grad /
+ * hrf_camera_calib_grad writes one contiguous gradient record of C cameras, 4-byte words:
+ *   [pose_grad C x 6 float | intrinsics_grad C x 4 float | ray_count C int32 | error 1 int32]
+ * (the intrinsics part is unused without intrinsics).  Every rank then takes the same step from all W records, either
+ * read from the peers' memory or gathered into one [W, record] tensor: the two give the same bits.
+ *   gradient g_c = (sum over r = 0..W-1, in rank order, of (double)grad_r[c]) / W, in float64 (W = 1: the single-rank
+ *                  step's input exactly, so hrf_camera_pose_step / hrf_camera_calib_step's bits);
+ *   a camera moves iff some rank's ray_count[c] > 0 and it is not fixed (the union of the ranks' batches);
+ *   if any rank's error word is non-zero, nothing is written, and a rank that sees bit 0 (a bad camera number) in
+ *   another rank's word sets bit 1 of its own `error` word (sticky, like bit 0).
+ * Adam, tables, origins, rotations and this rank's pool slots as hrf_camera_pose_step / hrf_camera_calib_step.
+ * ---------------------------------------------------------------------------------------- */
+/* Bytes of one gradient record for `num_cameras` cameras (11 C + 1 words), or -1 outside [1, 1024]. */
+int64_t hrf_camera_grad_record_bytes(int num_cameras);
+typedef struct {
+  const void* record[HRF_DP_MAX_WORLD];   /* every rank's record, rank order (device addresses this device can read) */
+  int32_t world, rank;                    /* W in [1, 8]; this rank */
+} hrf_camera_grad_records;
+/* One single-CTA launch; `error` is this rank's own sticky error word (in p2p, the error word of its own record). */
+int hrf_camera_pose_step_ranks(const hrf_camera_poses* poses, const hrf_camera_grad_records* records /* host */,
+                               int32_t* error /* [1] */, double lr, double beta1, double beta2, double eps,
+                               void* stream);
+int hrf_camera_calib_step_ranks(const hrf_camera_poses* poses, const hrf_camera_intrinsics* intrinsics,
+                                const hrf_camera_grad_records* records /* host */, int32_t* error /* [1] */, double lr,
+                                double lr_intrinsics, double beta1, double beta2, double eps, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Pre-processing that feeds the hot path (SURVEY 8f-4).
  * hrf_occupancy_from_masks: visual-hull carving, replaces occupancy_grid_generation_native.generate_from_masks
  * (actorshq/toolbox/native/occupancy_grid_generation.cu:16-123).  projection_matrices [C,4,4] are stored transposed
