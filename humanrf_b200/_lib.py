@@ -83,6 +83,11 @@ class CameraGradRecords(C.Structure):
     _fields_ = [("record", vp * DP_MAX_WORLD), ("world", i32), ("rank", i32)]
 
 
+class CameraResponses(C.Structure):
+    _fields_ = [("params", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("step", vp), ("fixed", vp), ("table", vp),
+                ("num_cameras", i32)]
+
+
 class DpTensor(C.Structure):
     _fields_ = [("param", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("grad_offset", i64), ("shadow_offset", i64),
                 ("local_shadow_bf16", vp), ("blob_perm", vp), ("active", vp), ("step", vp), ("n", i64),
@@ -140,6 +145,16 @@ _SIGNATURES = {
     "hrf_camera_calib_step_ranks": (C.c_int, [C.POINTER(CameraPoses), C.POINTER(CameraIntrinsics),
                                               C.POINTER(CameraGradRecords), vp, C.c_double, C.c_double, C.c_double,
                                               C.c_double, C.c_double, vp]),
+    "hrf_train_loss_response_workspace_bytes": (i64, [C.c_int]),
+    "hrf_camera_response_record_bytes": (i64, [C.c_int]),
+    "hrf_train_loss_response": (C.c_int, [vp, vp, vp, vp, vp, i64, vp, C.c_int, f32, f32, vp, vp, vp, vp, vp, vp, vp,
+                                          vp, vp]),
+    "hrf_camera_response_step": (C.c_int, [C.POINTER(CameraResponses), vp, vp, vp, C.c_double, C.c_double, C.c_double,
+                                           C.c_double, vp]),
+    "hrf_camera_response_step_ranks": (C.c_int, [C.POINTER(CameraResponses), C.POINTER(CameraGradRecords), vp,
+                                                 C.c_double, C.c_double, C.c_double, C.c_double, vp]),
+    "hrf_camera_response_write_table": (C.c_int, [C.POINTER(CameraResponses), vp]),
+    "hrf_camera_response_apply": (C.c_int, [vp, vp, i64, vp, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_forward": (C.c_int, [vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_backward": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),

@@ -34,7 +34,7 @@
 // as the single-rank kernels.
 #include <type_traits>
 
-#include "common.cuh"
+#include "camera_common.cuh"
 
 namespace hrf {
 
@@ -58,26 +58,6 @@ struct CalibSlot {                             // 48 bytes: the pose's 6 sums, t
 __host__ __device__ inline int pose_blocks(int64_t num_rays) {
   const int64_t b = (num_rays + kPoseRaysPerBlock - 1) / kPoseRaysPerBlock;
   return (int)(b < kPoseMaxBlocks ? b : kPoseMaxBlocks);
-}
-
-// Sum of x over the lanes of `peers` (this lane included), left in the lowest lane of `peers`.  A tree over the peers'
-// ranks: round k adds the partial 2^k ranks up.  Every lane of the warp runs every round.
-template <int N>
-__device__ __forceinline__ void reduce_peers(unsigned peers, float (&x)[N]) {
-  const int lane = threadIdx.x & 31;
-  int rank = __popc(peers & ((1u << lane) - 1u));
-  unsigned above = peers & ~((2u << lane) - 1u);
-  while (__any_sync(0xffffffffu, above != 0)) {
-    const int next = __ffs(above);                     // 1-based; 0 = none
-    const int src = next ? next - 1 : lane;
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      const float t = __shfl_sync(0xffffffffu, x[k], src);
-      if (next) x[k] += t;
-    }
-    above &= __ballot_sync(0xffffffffu, (rank & 1) == 0);
-    rank >>= 1;
-  }
 }
 
 __global__ void __launch_bounds__(kPoseThreads) pose_partials_kernel(
@@ -284,17 +264,6 @@ __global__ void __launch_bounds__(128) calib_finish_kernel(const CalibSlot* __re
                                                            float* __restrict__ intrinsics_grad,
                                                            int32_t* __restrict__ ray_count) {
   pose_finish_body<true>(partials, num_blocks, num_cameras, omega, alpha, pose_grad, intrinsics_grad, ray_count);
-}
-
-// One torch.optim.Adam update of x: m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g g, x -= lr / bc1 * m / (sqrt(v) / bc2s + eps)
-// in float64, every rounding spelled out.  Left to the compiler, which products are fused into an FMA depends on the
-// kernel around the update, and every step kernel must give the same bits from the same gradient.
-__device__ __forceinline__ void adam_update(double g, double& m_io, double& v_io, double& x, double lr_bc1, double bc2s,
-                                            double beta1, double beta2, double eps) {
-  const double m = __fma_rn(m_io, beta1, __dmul_rn(1.0 - beta1, g));
-  const double v = __fma_rn(v_io, beta2, __dmul_rn(__dmul_rn(1.0 - beta2, g), g));
-  m_io = m, v_io = v;
-  x = __fma_rn(-lr_bc1, m / (sqrt(v) / bc2s + eps), x);
 }
 
 // Adam on camera c's (omega, tau) at lr and, with kCalib, on its (alpha, beta) at lr_intrinsics with the same step

@@ -134,7 +134,8 @@ def write_metric_tables(out_dir, scores) -> None:
 
 @torch.no_grad()
 def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_frames: bool = True,
-                      render_step_size: float = 4e-4, rays_per_batch: int = 262144, lpips_weights=None):
+                      render_step_size: float = 4e-4, rays_per_batch: int = 262144, lpips_weights=None,
+                      camera_responses=None):
     """Renders every (camera_number, frame_number) of `pairs` with `model` through `loader`'s cameras (the colour of
     ``render_depth_map``), quantises it to 8 bits as ``Trainer.test`` does and scores it against the dataset's image and
     mask with ``image_metrics``.  With `save_frames` the views are written as ``out_dir/test_frames/<cam>_rgb%06d.png``
@@ -145,7 +146,10 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
     a view without a score (empty mask, or an ROI under 7x7 pixels) raises before the tables are written.  With
     `lpips_weights` (``load_lpips_alex``) each view's LPIPS is computed too, on the quantised render against the dataset
     image over the ROI ``image_metrics`` wrote, and the tables gain evaluate.py's LPIPS column; an ROI under 31x31 pixels
-    has no LPIPS and raises.  Returns a ``ViewScore`` per pair."""
+    has no LPIPS and raises.  With `camera_responses` (``toolbox.camera_response.CameraResponses`` learnt with the model),
+    a view whose camera has a learnt response is scored through it (``CameraResponses.apply`` with the render's alpha and
+    background 0), so the canonical radiance is compared with what that camera recorded; other views are scored as
+    rendered.  Returns a ``ViewScore`` per pair."""
     from .learned_occupancy import bake_occupancy_grid
     from .lpips import lpips
 
@@ -153,6 +157,7 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
     if not pairs:
         raise RuntimeError("no (camera, frame) pairs to evaluate")
     views = _Views(model, loader, render_step_size, rays_per_batch)
+    learned = camera_responses.learned().cpu() if camera_responses is not None else None
     dev = views.device
     values = torch.empty(len(pairs), 2 if lpips_weights is None else 3, dtype=torch.float64, device=dev)
     rois = []
@@ -163,7 +168,11 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
         if frame not in grids:
             grid = views.hull(frame)
             grids[frame] = bake_occupancy_grid(model, frame, grid, render_step_size) if bake else grid
-        pred = quantize(views.render(c, frame, grids[frame]).color)
+        view = views.render(c, frame, grids[frame])
+        color = view.color
+        if camera_responses is not None and bool(learned[c]):
+            color = camera_responses.apply(color.contiguous().clone(), view.alpha.contiguous(), c)
+        pred = quantize(color)
         gt, mask = ground_truth(loader, c, frame)
         gt = torch.from_numpy(gt).to(dev)
         _, roi = image_metrics(pred, gt, torch.from_numpy(mask).to(dev), out=values[k, :2])

@@ -32,6 +32,12 @@ sampler tables (hrf_camera_pose_step).  Data parallel (DESIGN.md §3.16): every 
 by every rank -- over NVLink between the exchange's two barriers ("p2p") or gathered after the bucket all-reduce
 ("nccl") -- and one step kernel (hrf_camera_pose_step_ranks) reduces them in rank order, so every replica takes the same
 pose step.  Without camera_poses, or before its start step, the step is unchanged.
+
+Camera colour responses (`camera_responses=`, toolbox/camera_response.py CameraResponses, DESIGN.md §3.17): from their
+start step on, the loss runs through each ray's camera response (hrf_train_loss_response, which also reduces the response
+gradient per camera), and after the field's Adam, where the pose step runs, the per-camera Adam on the responses
+(hrf_camera_response_step).  Data parallel: their gradient record travels as the pose record does.  Without
+camera_responses, or before their start step, the step launches exactly the kernels it launches without them.
 """
 from __future__ import annotations
 
@@ -66,20 +72,25 @@ class FusedTrainer:
                  max_steps: int = 50001, bce_loss_weight: float = 1e-3, huber_delta: float = 0.01,
                  render_step_size: float = 4e-4, world_size: int = 1, process_group=None, prune: bool = True,
                  seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False,
-                 camera_poses=None):
+                 camera_poses=None, camera_responses=None):
         """camera_poses: a toolbox.camera_refinement.CameraPoses over the loader the batches come from; its cameras'
         poses are refined with the field (then step() needs `cameras`).  Its world_size must be this trainer's: with
         world_size > 1 every rank builds its own CameraPoses over its own loader, the ranks exchange their per-camera
         gradient records and every rank takes the same pose step (DESIGN.md §3.16).  overlap_exchange=True does not
-        take camera_poses with world_size > 1 (ValueError)."""
-        if camera_poses is not None:
-            if getattr(camera_poses, "world_size", None) != world_size:
-                raise ValueError(f"camera_poses was built for world_size {getattr(camera_poses, 'world_size', None)}, "
+        take camera_poses with world_size > 1 (ValueError).
+        camera_responses: a toolbox.camera_response.CameraResponses over the same loader; each camera's colour response
+        is refined with the field (then step() needs `cameras`).  The same world_size, process_group and
+        overlap_exchange rules as camera_poses."""
+        for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses)):
+            if calib is None:
+                continue
+            if getattr(calib, "world_size", None) != world_size:
+                raise ValueError(f"{name} was built for world_size {getattr(calib, 'world_size', None)}, "
                                  f"the trainer has world_size {world_size}")
-            if world_size > 1 and getattr(camera_poses, "process_group", None) is not process_group:
-                raise ValueError("camera_poses was built over another process_group than the trainer's")
+            if world_size > 1 and getattr(calib, "process_group", None) is not process_group:
+                raise ValueError(f"{name} was built over another process_group than the trainer's")
             if world_size > 1 and overlap_exchange:
-                raise ValueError("camera_poses with world_size > 1 needs overlap_exchange=False")
+                raise ValueError(f"{name} with world_size > 1 needs overlap_exchange=False")
         if reuse not in ("none", "feat", "feat+grid"):
             raise ValueError("reuse must be 'none', 'feat' or 'feat+grid'")
         if exchange not in ("p2p", "nccl"):
@@ -88,15 +99,16 @@ class FusedTrainer:
         self.lr_decay, self.max_steps = lr_decay, max_steps
         self.bce_w, self.delta, self.step_size = bce_loss_weight, huber_delta, render_step_size
         self.world, self.pg, self.prune, self.reuse = world_size, process_group, prune, reuse
-        self.camera_poses = camera_poses
+        self.camera_poses, self.camera_responses = camera_poses, camera_responses
         self.exchange = exchange if world_size > 1 else "local"
         # exchange="p2p", optional: run the exchange of hash grid k (barrier + reduce/Adam/shadow kernel on a side stream)
         # while grid k+1 is still being scattered.  The exposed exchange shrinks, but four per-grid scatter launches cost
         # more than one: off by default.
         self.overlap_exchange = bool(overlap_exchange) and self.exchange == "p2p"
         self.rank = dist.get_rank(process_group) if world_size > 1 else 0
-        if camera_poses is not None and camera_poses.rank != self.rank:
-            raise ValueError(f"camera_poses has rank {camera_poses.rank}, the trainer rank {self.rank}")
+        for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses)):
+            if calib is not None and calib.rank != self.rank:
+                raise ValueError(f"{name} has rank {calib.rank}, the trainer rank {self.rank}")
         self.params: List[torch.nn.Parameter] = model.hot_parameters()
         dev = self.params[0].device
         self.dev = dev
@@ -141,8 +153,11 @@ class FusedTrainer:
         if self.world > 1:
             self._bar = torch.zeros(1, dtype=torch.float32, device=dev)
             self._side = torch.cuda.Stream(dev)
+        self.peer_records = []       # (this rank's record, every rank's address of it) to close, exchange="p2p"
         if camera_poses is not None and self.world > 1:
-            self._adopt_pose_records(camera_poses)
+            self.pose_records, self.pose_gather = self._adopt_grad_records(camera_poses)
+        if camera_responses is not None and self.world > 1:
+            self.response_records, self.response_gather = self._adopt_grad_records(camera_responses)
 
     # ---------------------------------------------------------------------------------------------- set-up
     def _peer_buffer(self, nbytes: int) -> torch.Tensor:
@@ -187,17 +202,19 @@ class FusedTrainer:
         self.peer_grad = self._exchange_handles(self.grad)
         self.peer_shadow = self._exchange_handles(self.shadow_flat)
 
-    def _adopt_pose_records(self, poses) -> None:
-        """Where every rank's pose-gradient record is read from.  p2p: the record moves into peer-visible memory and the
-        ranks' addresses are exchanged once; nccl: the records are gathered into one local [world, record] tensor."""
-        nbytes = int(poses.record.numel())
+    def _adopt_grad_records(self, owner):
+        """Where every rank's per-camera gradient record (`owner.record`: CameraPoses or CameraResponses) is read from.
+        p2p: the record moves into peer-visible memory and the ranks' addresses are exchanged once; nccl: the records
+        are gathered into one local flat [world * record] tensor.  Returns (every rank's record address in rank order, the
+        gather tensor or None)."""
+        nbytes = int(owner.record.numel())
         if self.exchange == "p2p":
-            poses._adopt_record(self._peer_buffer(nbytes))
-            self.peer_pose_record = self._exchange_handles(poses.record)
-            self.pose_records = list(self.peer_pose_record)
-        else:
-            self.pose_gather = torch.zeros((self.world, nbytes), dtype=torch.uint8, device=self.dev)
-            self.pose_records = [self.pose_gather[r].data_ptr() for r in range(self.world)]
+            owner._adopt_record(self._peer_buffer(nbytes))
+            peers = self._exchange_handles(owner.record)
+            self.peer_records.append(peers)
+            return list(peers), None
+        gather = torch.zeros(self.world * nbytes, dtype=torch.uint8, device=self.dev)    # flat: any backend's layout
+        return [gather[r * nbytes:].data_ptr() for r in range(self.world)], gather
 
     def _build_descriptors(self) -> None:
         m, nat, S = self.model, self.nat, self.model.num_segments
@@ -292,9 +309,12 @@ class FusedTrainer:
         lib, nat, dev = L.lib(), self.model.native(), t.device
         launches = 0
         poses = self.camera_poses if (self.camera_poses is not None and self.camera_poses.active(self.t)) else None
-        if poses is not None:
+        resp = (self.camera_responses if (self.camera_responses is not None and self.camera_responses.active(self.t))
+                else None)
+        if poses is not None or resp is not None:
             if cameras is None:
-                raise ValueError("camera_poses: step() needs the camera of every ray (`cameras`, int32 [R])")
+                raise ValueError(f"{'camera_poses' if poses is not None else 'camera_responses'}: step() needs the "
+                                 "camera of every ray (`cameras`, int32 [R])")
             cameras = L.require_cuda(cameras.reshape(-1), "cameras", torch.int32)
             if cameras.numel() != num_rays:
                 raise ValueError(f"cameras holds {cameras.numel()} entries for {num_rays} rays")
@@ -389,9 +409,13 @@ class FusedTrainer:
             loss_scale = (float(self.world * num_rays) / head[:1].clamp(min=1.0)).contiguous()
             if used is not None:
                 self.active_dev.copy_(head[1:] > 0)
-        L.check(lib.hrf_train_loss(color.data_ptr(), wsum.data_ptr(), rgba.data_ptr(), bg.data_ptr(), num_rays, self.delta,
-                                   self.bce_w, L.ptr(loss_scale), d_color.data_ptr(), d_wsum.data_ptr(), loss.data_ptr(),
-                                   L.stream()))
+        if resp is None:
+            L.check(lib.hrf_train_loss(color.data_ptr(), wsum.data_ptr(), rgba.data_ptr(), bg.data_ptr(), num_rays,
+                                       self.delta, self.bce_w, L.ptr(loss_scale), d_color.data_ptr(), d_wsum.data_ptr(),
+                                       loss.data_ptr(), L.stream()))
+        else:
+            launches += resp.loss(color, wsum, rgba, bg, cameras, num_rays, self.delta, self.bce_w, loss_scale, d_color,
+                                  d_wsum, loss) - 1
         # ---- backward: compositing, then the fused field backward into the flat bucket (clean: Adam re-zeroes it)
         d_sigma = torch.empty(n_cap, dtype=torch.float32, device=dev)
         d_rgb = torch.empty((n_cap, 3), dtype=torch.float32, device=dev)
@@ -434,19 +458,23 @@ class FusedTrainer:
                                               num_rays, g_o.data_ptr(), g_d.data_ptr(), None, L.stream()))
                 launches += 2 + poses.accumulate(g_o, g_d, d, cameras, num_rays)
                 mark("pose_grad")
-            launches += self._exchange_and_adam(poses if self.world > 1 else None, t_done)
+            launches += self._exchange_and_adam(poses if self.world > 1 else None, t_done,
+                                                resp if self.world > 1 else None)
             mark("exchange+adam")
             if poses is not None and self.world == 1:
                 launches += poses.step(t_done)
                 mark("pose_step")
+            if resp is not None and self.world == 1:
+                launches += resp.step(t_done)
+                mark("response_step")
         self.last = {"samples": count[0] if count is not None else n_cap, "loss": loss[0], "marks": marks}
         if return_loss:
             return float(loss.item())
         return launches
 
-    def _exchange_and_adam(self, poses=None, t_done: int = 0) -> int:
-        """The field's exchange and Adam; with `poses` (world_size > 1) also the pose step, which reads every rank's
-        gradient record."""
+    def _exchange_and_adam(self, poses=None, t_done: int = 0, responses=None) -> int:
+        """The field's exchange and Adam; with `poses` / `responses` (world_size > 1) also their steps, which read every
+        rank's gradient record."""
         lib = L.lib()
         lr = self.current_lr()
         self.t += 1
@@ -459,11 +487,16 @@ class FusedTrainer:
             dist.all_reduce(self.grad, group=self.pg)
             if poses is not None:
                 dist.all_gather_into_tensor(self.pose_gather, poses.record, group=self.pg)
+            if responses is not None:
+                dist.all_gather_into_tensor(self.response_gather, responses.record, group=self.pg)
             L.check(lib.hrf_adam_multi(self.adam_desc.data_ptr(), len(self.params), self.adam_blocks, lr, b1, b2, self.eps,
                                        1.0 / self.world, 1, L.stream()))
+            launches = 3
             if poses is not None:
-                return 4 + poses.step(t_done, self.pose_records)
-            return 3
+                launches += 1 + poses.step(t_done, self.pose_records)
+            if responses is not None:
+                launches += 1 + responses.step(t_done, self.response_records)
+            return launches
         # barrier A: every rank's gradients are complete
         dist.all_reduce(self._bar, group=self.pg)
         L.check(lib.hrf_dp_reduce_adam(C.byref(self.peers), self.adam_desc.data_ptr(), len(self.params), 0, self.adam_blocks, 1, lr,
@@ -474,7 +507,10 @@ class FusedTrainer:
             # fast peer from starting its next step's accumulate() (which rewrites its record) while this rank is still
             # reading it.
             launches += poses.step(t_done, self.pose_records)
-        # barrier B: every peer has read this rank's bucket (and pose record) and written this rank's shadow slices
+        if responses is not None:
+            # the same for the response record, which the next step's loss kernel rewrites
+            launches += responses.step(t_done, self.response_records)
+        # barrier B: every peer has read this rank's bucket (and gradient records) and written this rank's shadow slices
         dist.all_reduce(self._bar, group=self.pg)
         self.grad.zero_()
         return launches
@@ -523,6 +559,6 @@ class FusedTrainer:
                 if r != self.rank:
                     lib.hrf_peer_close(self.peer_grad[r])
                     lib.hrf_peer_close(self.peer_shadow[r])
-                    if self.camera_poses is not None:
-                        lib.hrf_peer_close(self.peer_pose_record[r])
+                    for peers in self.peer_records:
+                        lib.hrf_peer_close(peers[r])
             self._peer_ptrs = []      # the buffers themselves stay alive as long as tensors view them (process lifetime)

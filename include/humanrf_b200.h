@@ -510,6 +510,61 @@ int hrf_camera_calib_step_ranks(const hrf_camera_poses* poses, const hrf_camera_
                                 double lr_intrinsics, double beta1, double beta2, double eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Per-camera colour response refined with the field (toolbox/camera_response.py CameraResponses, DESIGN.md §3.17).
+ * Camera c carries a per-channel log gain gamma_c and offset b_c.  With w = weights_sum and fg = color - (1 - w) bg:
+ *   pred = color + expm1(gamma) fg + w b   (= e^gamma fg + w b + (1 - w) bg; the background was never seen by a camera)
+ * The loss kernel reads the response table [C,6] = ((float)expm1(gamma) x 3, (float)b x 3), written by the step kernels
+ * (and by the caller for the initial state).  A channel with em = b = 0 is the identity bit for bit.
+ * Gradient record of C cameras, 4-byte words: [response_grad C x 6 float | ray_count C int32 | error 1 int32]. */
+int64_t hrf_train_loss_response_workspace_bytes(int num_cameras);    /* -1 outside [1, 1024] */
+int64_t hrf_camera_response_record_bytes(int num_cameras);           /* (7 C + 1) * 4, -1 outside [1, 1024] */
+/* Two launches.  hrf_train_loss's loss, d_color and d_weights_sum with pred in place of color for the Huber term (the BCE
+ * term unchanged), at the response of each ray's camera and the same loss_scale_dev: d_color = g dpred with g = 1 + em,
+ * d_weights_sum = the BCE term + sum_k dpred_k (em_k bg_k + b_k).  At identity the outputs are hrf_train_loss's bytes,
+ * and the loss takes hrf_train_loss's addends (one atomicAdd per 256 rays, summed by the same tree).  response_grad[c] =
+ * (g_k sum_r dpred_k fg_k, sum_r dpred_k w) per channel, summed in a fixed order (the lane tree of hrf_camera_pose_grad,
+ * blocks in order, float64 across blocks), and ray_count[c]; written for every camera.  Two runs write identical bytes
+ * (loss_out aside: atomics).  A camera number outside [0, num_cameras) sets bit 0 of error[0]; that ray takes the
+ * identity and stays out of the sums.  No host synchronisation. */
+int hrf_train_loss_response(const float* color /* [R,3] */, const float* weights_sum /* [R] */,
+                            const float* rgba /* [R,4] */, const float* background /* [R,3] */,
+                            const int32_t* camera_numbers /* [R] */, int64_t num_rays,
+                            const float* response_table /* [C,6] */, int num_cameras, float huber_delta,
+                            float bce_weight, const float* loss_scale_dev, float* d_color /* [R,3] */,
+                            float* d_weights_sum /* [R] */, float* loss_out /* [1] accumulated into, or NULL */,
+                            float* response_grad /* [C,6] */, int32_t* ray_count /* [C] */, int32_t* error /* [1] */,
+                            void* workspace, void* stream);
+typedef struct {
+  double* params;                     /* [C,6] (gamma rgb, b rgb) */
+  double* exp_avg;                    /* [C,6] */
+  double* exp_avg_sq;                 /* [C,6] */
+  int32_t* step;                      /* [C] Adam step per camera */
+  const uint8_t* fixed;               /* [C] non-zero: the camera is never moved */
+  float* table;                       /* [C,6] rewritten for every camera that moves: (expm1(gamma), b) rounded once */
+  int num_cameras;                    /* C, 1..1024 */
+} hrf_camera_responses;
+/* One single-CTA launch: torch.optim.Adam (float64, roundings spelled out as hrf_camera_pose_step's) on (gamma_c, b_c)
+ * of every camera with ray_count[c] > 0 that is not fixed, then its table row.  Other cameras keep parameters, moments,
+ * step counter and table.  When error is non-NULL and error[0] != 0, nothing is written.  No host read. */
+int hrf_camera_response_step(const hrf_camera_responses* responses, const float* response_grad /* [C,6] */,
+                             const int32_t* ray_count /* [C] */, const int32_t* error /* [1] or NULL */, double lr,
+                             double beta1, double beta2, double eps, void* stream);
+/* Data parallel: the step on (sum over r = 0..W-1, in rank order, of (double)response_grad_r) / W, a camera moving iff
+ * some rank's ray_count > 0 and it is not fixed; the error rule of hrf_camera_pose_step_ranks (records in the response
+ * record's layout, `error` this rank's own sticky word).  W = 1 gives hrf_camera_response_step's bits. */
+int hrf_camera_response_step_ranks(const hrf_camera_responses* responses, const hrf_camera_grad_records* records /* host */,
+                                   int32_t* error /* [1] */, double lr, double beta1, double beta2, double eps,
+                                   void* stream);
+/* Rewrites the table row of every camera from its params, with the step kernels' expression (expm1 in float64, rounded
+ * once): after parameters are loaded, the table is the one the step would have written.  No host read. */
+int hrf_camera_response_write_table(const hrf_camera_responses* responses, void* stream);
+/* Applies camera `camera`'s response (its row of response_table) to a rendered image in place: color = color +
+ * em (color - (1 - alpha) background) + alpha b per channel.  Identity leaves the bytes unchanged. */
+int hrf_camera_response_apply(float* color /* [P,3] */, const float* alpha /* [P] */, int64_t num_pixels,
+                              const float* response_table /* [C,6] */, int camera, int num_cameras,
+                              const float* background /* [3] device */, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Pre-processing that feeds the hot path (SURVEY 8f-4).
  * hrf_occupancy_from_masks: visual-hull carving, replaces occupancy_grid_generation_native.generate_from_masks
  * (actorshq/toolbox/native/occupancy_grid_generation.cu:16-123).  projection_matrices [C,4,4] are stored transposed
