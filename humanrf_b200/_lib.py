@@ -155,6 +155,10 @@ _SIGNATURES = {
                                                  C.c_double, C.c_double, C.c_double, C.c_double, vp]),
     "hrf_camera_response_write_table": (C.c_int, [C.POINTER(CameraResponses), vp]),
     "hrf_camera_response_apply": (C.c_int, [vp, vp, i64, vp, C.c_int, C.c_int, vp, vp]),
+    "hrf_response_fit_workspace_bytes": (i64, [i64]),
+    "hrf_response_fit_accumulate": (C.c_int, [vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp]),
+    "hrf_response_fit_solve": (C.c_int, [C.POINTER(CameraResponses), vp, vp, C.c_int, C.c_double, C.c_double, vp, vp,
+                                         vp]),
     "hrf_compose_tensors_forward": (C.c_int, [vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_backward": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),

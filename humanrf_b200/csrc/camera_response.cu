@@ -1,5 +1,6 @@
 // Per-camera colour response refined with the field in the fused train step (hrf_train_loss_response,
-// hrf_camera_response_step, hrf_camera_response_step_ranks, hrf_camera_response_apply; DESIGN.md §3.17).
+// hrf_camera_response_step, hrf_camera_response_step_ranks, hrf_camera_response_apply; DESIGN.md §3.17), and the
+// held-out fit of a camera's response against a frozen model (hrf_response_fit_accumulate, hrf_response_fit_solve; §3.18).
 //
 // Camera c carries a per-channel log gain gamma_c and offset b_c.  With fg = color - (1 - w) bg the ray's foreground
 // (w = weights_sum, bg the trainer's random background, never seen by a camera):
@@ -288,6 +289,159 @@ __global__ void __launch_bounds__(256) response_apply_kernel(float* __restrict__
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Held-out response fit (hrf_response_fit_accumulate, hrf_response_fit_solve; DESIGN.md §3.18).  Per camera and channel
+// the gain g and offset b minimising sum (g f + a b - y/255)^2 + lambda n ((g - 1)^2 + b^2) over the fit pixels, from
+// the moments row [n, S_aa, per channel: S_ff, S_fa, S_fy, S_ay, S_yy] (y the 8-bit colour as an integer).  Every
+// addend is exact in float64 (fp32 x fp32, fp32 x u8, u8 x u8), so the sums' only rounding is the summation itself.
+constexpr int kFitRow = 17;
+constexpr int kFitThreads = 256;
+constexpr int kFitPixelsPerBlock = 2048;
+constexpr int kFitMaxBlocks = 1024;
+
+__host__ __device__ inline int fit_blocks(int64_t num_pixels) {
+  const int64_t b = (num_pixels + kFitPixelsPerBlock - 1) / kFitPixelsPerBlock;
+  return (int)(b < kFitMaxBlocks ? b : kFitMaxBlocks);
+}
+
+// Grid-stride over the pixels (the grid depends on P alone), a thread's sums in pixel order, the warp butterfly, then
+// the warps in order: one partial row per block.
+__global__ void __launch_bounds__(kFitThreads) response_fit_partials_kernel(
+    const float* __restrict__ color, const float* __restrict__ alpha, const uint8_t* __restrict__ gt,
+    const uint8_t* __restrict__ mask, int64_t num_pixels, double* __restrict__ partials) {
+  __shared__ double warp_rows[kFitThreads / 32][kFitRow];
+  double s[kFitRow];
+#pragma unroll
+  for (int e = 0; e < kFitRow; ++e) s[e] = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * kFitThreads;
+  for (int64_t i = (int64_t)blockIdx.x * kFitThreads + threadIdx.x; i < num_pixels; i += stride) {
+    if (__ldg(mask + i) == 0) continue;
+    const double a = (double)__ldg(alpha + i);
+    s[0] += 1.0;
+    s[1] += a * a;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const double f = (double)__ldg(color + 3 * i + k), y = (double)__ldg(gt + 3 * i + k);
+      s[2 + 5 * k] += f * f;
+      s[3 + 5 * k] += f * a;
+      s[4 + 5 * k] += f * y;
+      s[5 + 5 * k] += a * y;
+      s[6 + 5 * k] += y * y;
+    }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int e = 0; e < kFitRow; ++e) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) s[e] += __shfl_xor_sync(0xffffffffu, s[e], d);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int e = 0; e < kFitRow; ++e) warp_rows[warp][e] = s[e];
+  }
+  __syncthreads();
+  if (threadIdx.x < kFitRow) {
+    double t = warp_rows[0][threadIdx.x];
+#pragma unroll
+    for (int w = 1; w < kFitThreads / 32; ++w) t += warp_rows[w][threadIdx.x];
+    partials[(int64_t)blockIdx.x * kFitRow + threadIdx.x] = t;
+  }
+}
+
+// One warp: entry e of the blocks' partials in block order, then added into the camera's row.  A camera outside
+// [0, C) sets the error word and writes nothing.
+__global__ void __launch_bounds__(32) response_fit_finish_kernel(const double* __restrict__ partials, int num_blocks,
+                                                                 int camera, int num_cameras,
+                                                                 double* __restrict__ moments,
+                                                                 int32_t* __restrict__ error) {
+  if (camera < 0 || camera >= num_cameras) {
+    if (threadIdx.x == 0) atomicOr(error, 1);
+    return;
+  }
+  const int e = threadIdx.x;
+  if (e >= kFitRow || num_blocks == 0) return;
+  double t = partials[e];
+#pragma unroll 8
+  for (int b = 1; b < num_blocks; ++b) t += partials[(int64_t)b * kFitRow + e];
+  moments[(int64_t)camera * kFitRow + e] += t;
+}
+
+// The 2x2 ridge system of one channel by Cramer's rule, every operation rounded as written (no contraction), so that
+// a float64 restatement in the same order gives the same bits.  Returns (g, b); the data SSE at the identity and at
+// (g, b) come from the moments.
+struct FitChannel {
+  double g, b, sse_identity, sse_fit;
+};
+
+__device__ __forceinline__ FitChannel fit_channel(double n, double saa, const double* m, double lambda) {
+  const double inv255 = 1.0 / 255.0;
+  const double sff = m[0], sfa = m[1], sfy = __dmul_rn(m[2], inv255), say = __dmul_rn(m[3], inv255);
+  const double syy = __dmul_rn(__dmul_rn(m[4], inv255), inv255);
+  const double ln = __dmul_rn(lambda, n);
+  const double a11 = __dadd_rn(sff, ln), a22 = __dadd_rn(saa, ln), r1 = __dadd_rn(sfy, ln);
+  const double det = __dsub_rn(__dmul_rn(a11, a22), __dmul_rn(sfa, sfa));
+  FitChannel o;
+  o.g = __ddiv_rn(__dsub_rn(__dmul_rn(r1, a22), __dmul_rn(sfa, say)), det);
+  o.b = __ddiv_rn(__dsub_rn(__dmul_rn(a11, say), __dmul_rn(sfa, r1)), det);
+  // sum (f - y)^2 and sum (g f + a b - y)^2, expanded
+  o.sse_identity = __dadd_rn(__dsub_rn(sff, __dmul_rn(2.0, sfy)), syy);
+  double q = __dmul_rn(__dmul_rn(o.g, o.g), sff);
+  q = __dadd_rn(q, __dmul_rn(__dmul_rn(o.b, o.b), saa));
+  q = __dadd_rn(q, __dmul_rn(__dmul_rn(2.0, __dmul_rn(o.g, o.b)), sfa));
+  q = __dsub_rn(q, __dmul_rn(__dmul_rn(2.0, o.g), sfy));
+  q = __dsub_rn(q, __dmul_rn(__dmul_rn(2.0, o.b), say));
+  o.sse_fit = __dadd_rn(q, syy);
+  return o;
+}
+
+constexpr int kFitSolveThreads = 256;
+
+// One CTA.  Pass 1: every listed camera's three systems, its report and status.  Pass 2, only when every listed camera
+// succeeded: gamma = log g and b into params, then the camera's table row (the step kernels' expression).
+__global__ void __launch_bounds__(kFitSolveThreads) response_fit_solve_kernel(
+    hrf_camera_responses p, const double* __restrict__ moments, const int32_t* __restrict__ cameras, int K,
+    double lambda, double min_pixels, double* __restrict__ report, int32_t* __restrict__ status) {
+  int failed = 0;
+  for (int k = threadIdx.x; k < K; k += kFitSolveThreads) {
+    const int c = cameras[k];
+    double* rep = report + 8 * (int64_t)k;
+    int st = HRF_FIT_OK;
+    if (c < 0 || c >= p.num_cameras) {
+      st = HRF_FIT_BAD_CAMERA;
+#pragma unroll
+      for (int j = 0; j < 7; ++j) rep[j] = 0.0;
+    } else {
+      const double* row = moments + (int64_t)c * kFitRow;
+      const double n = row[0];
+      rep[0] = n;
+      if (n < min_pixels) st = HRF_FIT_TOO_FEW_PIXELS;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const FitChannel o = fit_channel(n, row[1], row + 2 + 5 * ch, lambda);
+        rep[1 + ch] = o.sse_identity;
+        rep[4 + ch] = o.sse_fit;
+        if (st == HRF_FIT_OK && !(isfinite(o.g) && isfinite(o.b))) st = HRF_FIT_NOT_FINITE;
+        if (st == HRF_FIT_OK && !(o.g > 0.0)) st = HRF_FIT_GAIN_NOT_POSITIVE;
+      }
+    }
+    rep[7] = (double)st;
+    status[k] = st;
+    failed |= st != HRF_FIT_OK;
+  }
+  if (__syncthreads_or(failed)) return;
+  for (int k = threadIdx.x; k < K; k += kFitSolveThreads) {
+    const int c = cameras[k];
+    const double* row = moments + (int64_t)c * kFitRow;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      const FitChannel o = fit_channel(row[0], row[1], row + 2 + 5 * ch, lambda);
+      p.params[6 * c + ch] = log(o.g);
+      p.params[6 * c + 3 + ch] = o.b;
+    }
+    response_table_row(p, c);
+  }
+}
+
 // Raises a kernel's dynamic shared-memory limit to `bytes` once per device (bit d of `done`), not on every call: the
 // attribute belongs to the device's context, and the loss kernel runs on every train step.
 static int opt_in_smem_once(std::atomic<uint64_t>& done, const void* kernel, int bytes) {
@@ -398,6 +552,52 @@ extern "C" int hrf_camera_response_write_table(const hrf_camera_responses* respo
   HRF_REQUIRE(p.num_cameras >= 1 && p.num_cameras <= kRespMaxCameras, "camera count outside [1, 1024]");
   HRF_REQUIRE(p.params != nullptr && p.table != nullptr, "null response table");
   response_table_kernel<<<(p.num_cameras + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  HRF_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int64_t hrf_response_fit_workspace_bytes(int64_t num_pixels) {
+  if (num_pixels < 0) return -1;
+  const int blocks = fit_blocks(num_pixels);
+  return (int64_t)(blocks > 0 ? blocks : 1) * kFitRow * (int64_t)sizeof(double);
+}
+
+extern "C" int hrf_response_fit_accumulate(const float* color, const float* alpha, const uint8_t* gt,
+                                           const uint8_t* mask, int64_t num_pixels, int camera, int num_cameras,
+                                           double* moments, int32_t* error, void* workspace, void* stream) {
+  HRF_REQUIRE(num_pixels >= 0, "negative pixel count");
+  HRF_REQUIRE(num_cameras >= 1 && num_cameras <= kRespMaxCameras, "camera count outside [1, 1024]");
+  HRF_REQUIRE(moments != nullptr && error != nullptr, "null argument");
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const bool valid = camera >= 0 && camera < num_cameras;
+  const int blocks = valid ? fit_blocks(num_pixels) : 0;
+  if (blocks > 0) {
+    HRF_REQUIRE(color && alpha && gt && mask && workspace, "null input");
+    response_fit_partials_kernel<<<blocks, kFitThreads, 0, st>>>(color, alpha, gt, mask, num_pixels,
+                                                                 reinterpret_cast<double*>(workspace));
+    HRF_CHECK_LAUNCH();
+  }
+  if (blocks > 0 || !valid) {
+    response_fit_finish_kernel<<<1, 32, 0, st>>>(reinterpret_cast<const double*>(workspace), blocks, camera,
+                                                 num_cameras, moments, error);
+    HRF_CHECK_LAUNCH();
+  }
+  return 0;
+}
+
+extern "C" int hrf_response_fit_solve(const hrf_camera_responses* responses, const double* moments,
+                                      const int32_t* cameras, int num_listed, double lambda, double min_pixels,
+                                      double* report, int32_t* status, void* stream) {
+  HRF_REQUIRE(responses != nullptr, "null argument");
+  const hrf_camera_responses& p = *responses;
+  HRF_REQUIRE(p.num_cameras >= 1 && p.num_cameras <= kRespMaxCameras, "camera count outside [1, 1024]");
+  HRF_REQUIRE(p.params != nullptr && p.table != nullptr, "null response table");
+  HRF_REQUIRE(num_listed >= 0 && num_listed <= kRespMaxCameras, "listed camera count outside [0, 1024]");
+  HRF_REQUIRE(lambda >= 0.0, "negative ridge");
+  if (num_listed == 0) return 0;
+  HRF_REQUIRE(moments && cameras && report && status, "null argument");
+  response_fit_solve_kernel<<<1, kFitSolveThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      p, moments, cameras, num_listed, lambda, min_pixels, report, status);
   HRF_CHECK_LAUNCH();
   return 0;
 }

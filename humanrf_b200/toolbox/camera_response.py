@@ -14,19 +14,76 @@ The Huber term of the loss is taken on pred - gt, the mask's BCE term is unchang
 gamma = b = 0 the loss kernel writes hrf_train_loss's bytes.  After the field's Adam, hrf_camera_response_step runs
 Adam (float64) on every camera that had rays and is not fixed.  The response exports as 6 numbers per camera
 (``gains()``, ``offsets()``, ``write_response_csv``) and can be applied to a render afterwards (``apply``).
+
+Cameras that were never trained (held-out test cameras) get their response from a closed-form least-squares fit
+against the frozen model on frames the evaluation does not score (``held_out_fit_pairs``,
+``CameraResponses.fit_held_out``, DESIGN.md §3.18).
 """
 from __future__ import annotations
 
 import csv
 import ctypes as C
 import hashlib
+import math
+from dataclasses import dataclass
 from typing import Iterable, Optional, Sequence
 
+import numpy as np
 import torch
 
 from .. import _lib as L
 
 RESPONSE_COLUMNS = ("name", "gain_r", "gain_g", "gain_b", "offset_r", "offset_g", "offset_b")
+FIT_COLUMNS = ("name", "fit_views", "n", "gain_r", "gain_g", "gain_b", "offset_r", "offset_g", "offset_b",
+               "psnr_before", "psnr_after")
+FIT_ROW = 17            # moments per camera: n, S_aa, per channel S_ff, S_fa, S_fy, S_ay, S_yy
+FIT_STATUS = {1: "fewer fit pixels than min_pixels", 2: "the fit is not finite (gain and offset cannot be told apart)",
+              3: "the fitted gain is not positive", 4: "camera outside the responses' cameras"}
+
+
+@dataclass
+class ResponseFit:
+    """One held-out camera's fit: its fit frames, the number of fit pixels, the gain and offset per channel, and the
+    masked PSNR (dB) of the float render against the dataset's colour over the fit pixels, before and after the fit."""
+    camera: int
+    frames: tuple
+    n: int
+    gain: tuple
+    offset: tuple
+    psnr_before: float
+    psnr_after: float
+
+
+def held_out_fit_pairs(score_pairs, frame_numbers, per_camera: int = 8) -> list:
+    """(camera, frame) pairs to fit held-out responses on: for each camera of `score_pairs` (in order of first
+    appearance), `per_camera` of `frame_numbers` spread evenly (``np.round(np.linspace(0, n - 1, per_camera))``, the
+    rounding of the ActorsHQ presets' ``get_spaced_elements``) over the frames that camera is NOT scored on, or all of
+    them when there are fewer.  No returned pair is a scored pair."""
+    if per_camera < 1:
+        raise ValueError(f"per_camera must be at least 1, got {per_camera}")
+    scored, order = {}, []
+    for c, f in score_pairs:
+        c = int(c)
+        if c not in scored:
+            scored[c] = set()
+            order.append(c)
+        scored[c].add(int(f))
+    frames = list(dict.fromkeys(int(f) for f in frame_numbers))
+    out = []
+    for c in order:
+        spare = [f for f in frames if f not in scored[c]]
+        if len(spare) <= per_camera:
+            picked = spare
+        else:
+            idx = np.round(np.linspace(0, len(spare) - 1, per_camera)).astype(int)
+            picked = [spare[i] for i in dict.fromkeys(idx.tolist())]
+        out.extend((c, f) for f in picked)
+    return out
+
+
+def _masked_psnr(sse: float, n: int) -> float:
+    mse = sse / (3 * n)
+    return math.inf if mse <= 0 else -10.0 * math.log10(mse)
 
 
 class CameraResponses:
@@ -86,6 +143,7 @@ class CameraResponses:
         p.params, p.exp_avg, p.exp_avg_sq = (t.data_ptr() for t in (self.params, self.exp_avg, self.exp_avg_sq))
         p.step, p.fixed, p.table, p.num_cameras = self.steps.data_ptr(), self.fixed.data_ptr(), self.table.data_ptr(), n
         self._desc = p
+        self.fits = {}          # camera -> ResponseFit of fit_held_out; not part of state_dict
         self.rank = 0
         if self.world_size > 1:
             import torch.distributed as dist
@@ -211,6 +269,141 @@ class CameraResponses:
                                                       int(camera), self.num_cameras, bg.data_ptr(), L.stream()))
         return color
 
+    # ---------------------------------------------------------------------------------------------- held-out fit
+    @property
+    def fitted_pairs(self) -> dict:
+        """camera -> the (camera, frame) pairs its held-out response was fitted on (``fit_held_out``)."""
+        return {c: [(c, f) for f in fit.frames] for c, fit in self.fits.items()}
+
+    def accumulate_fit(self, color, alpha, gt_u8, mask, camera: int, moments, error, workspace=None) -> None:
+        """Enqueues hrf_response_fit_accumulate: adds one view's sums (pixels where `mask` != 0) to row `camera` of
+        `moments` (float64 [C,17]).  `color` float32 [...,3], `alpha` float32 [...], `gt_u8` uint8 [...,3], `mask` uint8
+        or bool [...], all contiguous on the responses' device; `error` int32 [1]."""
+        if isinstance(mask, torch.Tensor) and mask.dtype == torch.bool:
+            mask = mask.view(torch.uint8)
+        for t, name, dt in ((color, "color", torch.float32), (alpha, "alpha", torch.float32), (gt_u8, "gt", torch.uint8),
+                            (mask, "mask", torch.uint8), (moments, "moments", torch.float64), (error, "error", torch.int32)):
+            L.require_cuda(t, name, dt)
+        P = alpha.numel()
+        if color.numel() != 3 * P or gt_u8.numel() != 3 * P or mask.numel() != P:
+            raise RuntimeError(f"color {tuple(color.shape)}, gt {tuple(gt_u8.shape)} and mask {tuple(mask.shape)} do not "
+                               f"match {P} pixels")
+        if tuple(moments.shape) != (self.num_cameras, FIT_ROW):
+            raise RuntimeError(f"moments must be [{self.num_cameras}, {FIT_ROW}], got {tuple(moments.shape)}")
+        lib = L.lib()
+        if workspace is None:
+            workspace = torch.empty(int(lib.hrf_response_fit_workspace_bytes(P)), dtype=torch.uint8, device=color.device)
+        with torch.cuda.device(color.device):
+            L.check(lib.hrf_response_fit_accumulate(color.data_ptr(), alpha.data_ptr(), gt_u8.data_ptr(),
+                                                    mask.data_ptr(), P, int(camera), self.num_cameras,
+                                                    moments.data_ptr(), error.data_ptr(), workspace.data_ptr(),
+                                                    L.stream()))
+
+    def solve_fit(self, moments, cameras, ridge: float = 1e-6, min_pixels: int = 1024):
+        """Enqueues hrf_response_fit_solve for `cameras` and returns (report float64 [K,8], status int32 [K]) on the
+        device: report rows (n, SSE at the identity rgb, SSE at the fit rgb, status).  Writes the listed cameras' params
+        and table rows only when every one of them succeeds."""
+        L.require_cuda(moments, "moments", torch.float64)
+        if tuple(moments.shape) != (self.num_cameras, FIT_ROW):
+            raise RuntimeError(f"moments must be [{self.num_cameras}, {FIT_ROW}], got {tuple(moments.shape)}")
+        cams = torch.as_tensor(list(cameras), dtype=torch.int32).to(self.device)
+        K = int(cams.numel())
+        report = torch.zeros((K, 8), dtype=torch.float64, device=self.device)
+        status = torch.zeros(K, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            L.check(L.lib().hrf_response_fit_solve(C.byref(self._desc), moments.data_ptr(), cams.data_ptr(), K,
+                                                   float(ridge), float(min_pixels), report.data_ptr(),
+                                                   status.data_ptr(), L.stream()))
+        return report, status
+
+    @torch.no_grad()
+    def fit_held_out(self, model, loader, pairs, *, ridge: float = 1e-6, min_pixels: int = 1024, bake: bool = False,
+                     render_step_size: float = 4e-4, rays_per_batch: int = 262144) -> list:
+        """Fits the response of every camera of `pairs` (camera, frame) against the frozen `model` (DESIGN.md §3.18).
+        Each pair is rendered as ``evaluate_sequence`` renders it (``_Views``, background 0, the frame's hull, or with
+        `bake` the hull baked once per frame) and its pixels inside the dataset's mask are added to the camera's moments;
+        one solve then gives, per channel, the gain g and offset b minimising sum (g f + a b - y)^2 +
+        ridge n ((g - 1)^2 + b^2) (f the render, a its alpha, y = gt / 255), written as gamma = log g and b.
+
+        Raises ``ValueError`` before any work for a fixed camera, a camera with a trained response (step counter > 0), a
+        frame that is not one of the model's or a loader whose camera count differs, and after the solve, naming the
+        camera and the reason, when a camera cannot be fitted (fewer than `min_pixels` pixels, a singular system, a gain
+        <= 0); nothing has been written then.  Fitting a camera again replaces its earlier fit.  Returns a
+        ``ResponseFit`` per camera, in camera order; ``fits`` and ``fitted_pairs`` keep them."""
+        from .depth_maps import _Views
+        from .evaluation import ground_truth
+        from .learned_occupancy import bake_occupancy_grid
+
+        n_loader = int(loader.all_inverse_krs.shape[0])
+        if n_loader != self.num_cameras:
+            raise ValueError(f"the loader has {n_loader} cameras, the responses {self.num_cameras}")
+        pairs = [(int(c), int(f)) for c, f in pairs]
+        if not pairs:
+            raise ValueError("no (camera, frame) pairs to fit on")
+        steps = self.steps.cpu().numpy()
+        for c, f in pairs:
+            if not 0 <= c < self.num_cameras:
+                raise ValueError(f"camera {c} outside [0, {self.num_cameras})")
+            if c in self.fixed_cameras:
+                raise ValueError(f"camera {c} is fixed: it holds the gauge and keeps the identity")
+            if steps[c] > 0:
+                raise ValueError(f"camera {c} has a trained response ({int(steps[c])} steps): a held-out fit would "
+                                 "replace it")
+            if f not in model.sorted_frame_numbers:
+                raise ValueError(f"frame {f} is not one of the model's frames")
+        cameras = sorted({c for c, _ in pairs})
+        dev = self.device
+        moments = torch.zeros((self.num_cameras, FIT_ROW), dtype=torch.float64, device=dev)
+        error = torch.zeros(1, dtype=torch.int32, device=dev)
+        views = _Views(model, loader, render_step_size, rays_per_batch)
+        grids = {}
+        for c, frame in pairs:
+            if frame not in grids:
+                grid = views.hull(frame)
+                grids[frame] = bake_occupancy_grid(model, frame, grid, render_step_size) if bake else grid
+            view = views.render(c, frame, grids[frame])
+            gt, mask = ground_truth(loader, c, frame)
+            self.accumulate_fit(view.color.contiguous(), view.alpha.contiguous(), torch.from_numpy(gt).to(dev),
+                                torch.from_numpy(mask).to(dev), c, moments, error)
+            del view
+        report, status = self.solve_fit(moments, cameras, ridge, min_pixels)
+        report, status = report.cpu().numpy(), status.cpu().numpy()
+        if int(error.cpu()[0]) != 0:
+            raise RuntimeError("hrf_response_fit_accumulate saw a camera outside the responses' cameras")
+        bad = [(c, int(s)) for c, s in zip(cameras, status) if s != 0]
+        if bad:
+            raise ValueError("held-out response fit refused, nothing written: " + "; ".join(
+                f"camera {c}: {FIT_STATUS.get(s, f'status {s}')} ({int(report[cameras.index(c), 0])} pixels)"
+                for c, s in bad))
+        params = self.params.cpu().numpy()
+        fits = []
+        for k, c in enumerate(cameras):
+            n = int(report[k, 0])
+            fit = ResponseFit(camera=c, frames=tuple(f for cc, f in pairs if cc == c), n=n,
+                              gain=tuple(float(x) for x in np.exp(params[c, :3])),
+                              offset=tuple(float(x) for x in params[c, 3:]),
+                              psnr_before=_masked_psnr(float(report[k, 1:4].sum()), n),
+                              psnr_after=_masked_psnr(float(report[k, 4:7].sum()), n))
+            self.fits[c] = fit
+            fits.append(fit)
+        return fits
+
+    def write_fit_csv(self, path, loader=None) -> None:
+        """One row per camera with a held-out fit (``fits``), in camera order: name (from `loader`'s cameras, by
+        default the responses' loader), fit views, fit pixels, gains, offsets, and the masked PSNR of the float render
+        over the fit pixels before and after the fit."""
+        from .camera_refinement import _camera_name
+
+        cams = getattr(self.loader if loader is None else loader, "cameras", None)
+        with open(path, "w", newline="") as fh:
+            w = csv.writer(fh)
+            w.writerow(FIT_COLUMNS)
+            for c in sorted(self.fits):
+                fit = self.fits[c]
+                name = _camera_name(cams[c], c) if cams is not None and c < len(cams) else f"Cam{c + 1:03d}"
+                w.writerow([name, len(fit.frames), fit.n] + [repr(float(x)) for x in (*fit.gain, *fit.offset)]
+                           + [repr(fit.psnr_before), repr(fit.psnr_after)])
+
     # ---------------------------------------------------------------------------------------------- state
     def _write_table(self) -> None:
         """Rebuilds the table from the parameters on the device, with the step kernels' expression
@@ -234,6 +427,7 @@ class CameraResponses:
             self.fixed.zero_()
             self.fixed[fixed] = 1
             self.fixed_cameras = tuple(fixed)
+        self.fits = {}          # the loaded parameters replace any held-out fit
         self._write_table()
 
     def write_response_csv(self, path) -> None:

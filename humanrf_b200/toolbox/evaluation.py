@@ -149,13 +149,21 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
     has no LPIPS and raises.  With `camera_responses` (``toolbox.camera_response.CameraResponses`` learnt with the model),
     a view whose camera has a learnt response is scored through it (``CameraResponses.apply`` with the render's alpha and
     background 0), so the canonical radiance is compared with what that camera recorded; other views are scored as
-    rendered.  Returns a ``ViewScore`` per pair."""
+    rendered.  Cameras with a held-out fit (``CameraResponses.fit_held_out``, in ``camera_responses.fitted_pairs``)
+    follow two more rules: a scored pair that is one of that camera's fit pairs raises ``ValueError`` before anything
+    is rendered or written, and the applied colour is clamped to [0, 1] before quantising, as a camera saturates at 255.
+    When a scored camera has a fit, ``out_dir/response_fit.csv`` records every fit (``write_fit_csv``): those scores come
+    from a protocol other than plain ActorsHQ.  Returns a ``ViewScore`` per pair."""
     from .learned_occupancy import bake_occupancy_grid
     from .lpips import lpips
 
     pairs = [(_check_camera(loader, c), _check_frame(model, f)) for c, f in pairs]
     if not pairs:
         raise RuntimeError("no (camera, frame) pairs to evaluate")
+    fitted = camera_responses.fitted_pairs if camera_responses is not None else {}
+    leaked = [(c, f) for c, f in pairs if c in fitted and (c, f) in fitted[c]]
+    if leaked:
+        raise ValueError(f"scored (camera, frame) {leaked} are among the pairs the held-out responses were fitted on")
     views = _Views(model, loader, render_step_size, rays_per_batch)
     learned = camera_responses.learned().cpu() if camera_responses is not None else None
     dev = views.device
@@ -172,6 +180,8 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
         color = view.color
         if camera_responses is not None and bool(learned[c]):
             color = camera_responses.apply(color.contiguous().clone(), view.alpha.contiguous(), c)
+        if c in fitted:
+            color = color.clamp(0.0, 1.0)
         pred = quantize(color)
         gt, mask = ground_truth(loader, c, frame)
         gt = torch.from_numpy(gt).to(dev)
@@ -192,4 +202,6 @@ def evaluate_sequence(model, loader, pairs, out_dir, bake: bool = False, save_fr
     if bad:
         raise RuntimeError(f"no LPIPS for (camera, frame) {bad}: a mask bounding box under 31x31 pixels")
     write_metric_tables(out_dir, scores)
+    if any(c in fitted for c, _ in pairs):
+        camera_responses.write_fit_csv(os.path.join(out_dir, "response_fit.csv"), loader)
     return scores

@@ -564,6 +564,33 @@ int hrf_camera_response_apply(float* color /* [P,3] */, const float* alpha /* [P
                               const float* response_table /* [C,6] */, int camera, int num_cameras,
                               const float* background /* [3] device */, void* stream);
 
+/* Held-out response fit (CameraResponses.fit_held_out, DESIGN.md §3.18).  Per camera and channel, the gain g and offset
+ * b minimising  sum over the fit pixels of (g f + a b - y / 255)^2 + lambda n ((g - 1)^2 + b^2)  with f the rendered
+ * colour, a its alpha (background 0) and y the dataset's 8-bit colour.  Moments row of a camera, float64 [17]:
+ *   [n, S_aa, then per channel r, g, b: S_ff, S_fa, S_fy, S_ay, S_yy]   (y the integer 0..255)
+ * Every addend is exact in float64, so the only rounding is the summation; n and S_yy are exact integers. */
+#define HRF_FIT_OK 0
+#define HRF_FIT_TOO_FEW_PIXELS 1      /* n < min_pixels */
+#define HRF_FIT_NOT_FINITE 2          /* a gain or offset is inf or NaN (a singular system) */
+#define HRF_FIT_GAIN_NOT_POSITIVE 3   /* g <= 0: log g cannot represent it */
+#define HRF_FIT_BAD_CAMERA 4          /* the listed camera is outside [0, C) */
+int64_t hrf_response_fit_workspace_bytes(int64_t num_pixels);       /* -1 for a negative count */
+/* Adds the sums of one view (the pixels with mask != 0) to row `camera` of moments [C,17].  Two launches: block
+ * partials from a grid that depends on P alone, then one block adding them in block order into the row.  No float
+ * atomics: a rerun writes the same bytes.  A camera outside [0, num_cameras) sets error[0] |= 1 and writes nothing;
+ * P = 0 writes nothing.  No host synchronisation. */
+int hrf_response_fit_accumulate(const float* color /* [P,3] */, const float* alpha /* [P] */,
+                                const uint8_t* gt /* [P,3] */, const uint8_t* mask /* [P] */, int64_t num_pixels,
+                                int camera, int num_cameras, double* moments /* [C,17] */, int32_t* error /* [1] */,
+                                void* workspace, void* stream);
+/* One CTA.  For each listed camera, the three 2x2 systems in float64 by Cramer's rule; report [K,8] = (n, SSE at the
+ * identity r g b, SSE at the fit r g b, status), the data SSEs from the moments, and status [K] (HRF_FIT_*).  When every
+ * listed camera succeeds, its params (gamma = log g, b) and table row are written and nothing else; otherwise no params
+ * or table row at all.  Moments, moments of Adam and step counters are never written.  No host read. */
+int hrf_response_fit_solve(const hrf_camera_responses* responses, const double* moments /* [C,17] */,
+                           const int32_t* cameras /* [K] */, int num_listed, double lambda, double min_pixels,
+                           double* report /* [K,8] */, int32_t* status /* [K] */, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Pre-processing that feeds the hot path (SURVEY 8f-4).
  * hrf_occupancy_from_masks: visual-hull carving, replaces occupancy_grid_generation_native.generate_from_masks
