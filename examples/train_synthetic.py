@@ -85,7 +85,9 @@ def psnr(a, b):
     return float(-10 * torch.log10(torch.mean((a - b) ** 2)))      # trainer.py:218-222
 
 
-def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet=False):
+def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet=False, return_state=False):
+    """Returns the held-out PSNR history [(step, dB)]; with `return_state` also a dict of the trained student, the
+    dataset, the occupancy grid, the camera-table builder, the frames and the held-out camera."""
     from humanrf_b200.dataset.occupancy_grid_native import OccupanyGrid
 
     dev = torch.device("cuda:0")
@@ -149,6 +151,9 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
             if not quiet:
                 print(f"step {step:5d}  loss {float(trainer.last['loss']):.5f}  samples {ib.num_samples}  rays {ib.num_rays}  "
                       f"held-out PSNR {history[-1][1]:.2f} dB  ({rays_done / (time.time() - t0):.0f} rays/s incl. validation)")
+    if return_state:
+        return history, dict(student=student, dataset=ds, occupancy_grid=og, tables=tables, frames=frames,
+                             held_out=held_out)
     return history
 
 

@@ -36,7 +36,11 @@ class Field(C.Structure):
     _fields_ = [("segments", vp), ("frame_to_segment", vp), ("frame_to_tlocal", vp), ("mlp_blob", vp),
                 ("level_scale", f32 * N_LEVELS), ("level_res", u32 * N_LEVELS), ("num_segments", i32),
                 ("lut_size", i32), ("vec_res", i32), ("density_scale", f32), ("camera_embeddings", vp),
-                ("camera_embedding_dim", i32), ("num_cameras", i32), ("color_in_width", i32)]
+                ("camera_embedding_dim", i32), ("num_cameras", i32), ("color_in_width", i32), ("table_format", i32)]
+
+
+TABLE_BF16X2, TABLE_INT8X2 = 0, 1     # hrf_field.table_format
+QUANT_CLIPS = 8
 
 
 class Samples(C.Structure):
@@ -164,6 +168,9 @@ _SIGNATURES = {
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),
     "hrf_cast_bf16": (C.c_int, [vp, vp, i64, vp]),
     "hrf_transpose_vectors": (C.c_int, [vp, vp, C.c_int, vp]),
+    "hrf_quantize_tables_select": (C.c_int, [C.POINTER(vp), C.POINTER(u32), C.POINTER(u32), C.c_int, vp, vp, vp, vp, vp]),
+    "hrf_quantize_tables_write": (C.c_int, [C.POINTER(vp), C.POINTER(u32), C.POINTER(u32), vp, C.POINTER(vp), vp]),
+    "hrf_quantize_fold_vectors": (C.c_int, [vp, vp, C.c_int, vp, vp]),
     "hrf_occupancy_from_masks": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "hrf_occupancy_union_count": (C.c_int, [vp, vp, i64, vp, vp]),
     "hrf_bake_occupancy_workspace_bytes": (i64, [C.c_int]),

@@ -371,6 +371,7 @@ static int field_backward_mlp(const hrf_field* f, const hrf_samples* s, const fl
                               const float* d_geo, const void* feat_bf16, const int32_t* feat_index, float* d_mlp,
                               float* d_camera_embeddings, float* d_directions, void* workspace, void* stream) {
   HRF_REQUIRE(f != nullptr && s != nullptr, "null argument");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2, "an int8 field (compact model) serves inference only: it has no gradients");
   HRF_REQUIRE(f->num_segments < 255, "at most 254 temporal segments");
   if (s->num_samples == 0) return 0;
   HRF_REQUIRE(workspace != nullptr, "hrf_field_backward needs a workspace of 160 bytes per sample");
@@ -446,6 +447,7 @@ extern "C" int hrf_field_backward_tables(const hrf_field* f, const hrf_samples* 
                                          const void* grid_feat_bf16, const int32_t* feat_index, int64_t grid_feat_stride,
                                          const void* workspace, int grid_first, int grid_count, void* stream) {
   HRF_REQUIRE(f != nullptr && s != nullptr && seg_grads != nullptr, "null argument");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2, "an int8 field (compact model) serves inference only: it has no gradients");
   HRF_REQUIRE(grid_first >= 0 && grid_count >= 1 && grid_first + grid_count <= 4, "grids are 0..3 (xyz, xyt, yzt, xzt)");
   // HRF_SCATTER = 6 (the default) | 5, read per call so that the tests can switch it: scatter_v6.cu, or scatter_v5.cu, v6's
   // reference in tests/test_scatter_gpu.py.  Any other value is an error: a stale setting must not time one generation
@@ -466,7 +468,8 @@ extern "C" int hrf_field_backward(const hrf_field* f, const hrf_samples* s, cons
                                   const float* d_sigma, const float* d_rgb, const float* d_geo, const void* feat_bf16,
                                   const void* grid_feat_bf16, const int32_t* feat_index, int64_t grid_feat_stride,
                                   float* d_mlp, float* d_camera_embeddings, void* workspace, void* stream) {
-  HRF_REQUIRE(seg_grads != nullptr, "null argument");
+  HRF_REQUIRE(f != nullptr && seg_grads != nullptr, "null argument");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2, "an int8 field (compact model) serves inference only: it has no gradients");
   if (int rc = hrf_field_backward_mlp(f, s, d_sigma, d_rgb, d_geo, feat_bf16, feat_index, d_mlp, d_camera_embeddings, workspace,
                                       stream))
     return rc;

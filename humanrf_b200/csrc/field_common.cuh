@@ -194,10 +194,24 @@ __device__ __forceinline__ void corner_weights(Cell a, Cell b, Cell c, float w[8
   }
 }
 
-// Trilinear gather of one level of one grid -> 2 features (fp32 blend of bf16 entries).
-__device__ __forceinline__ float2 gather_level(const uint32_t* __restrict__ tab, bool hashed, uint32_t res,
+// Table entry formats (hrf_field.table_format): how one entry of a grid is stored and turned into its two features.
+struct TabBf16x2 {   // HRF_TABLE_BF16X2: the bf16 shadow of the fp32 masters
+  using Entry = uint32_t;
+  __device__ __forceinline__ static float lo(Entry r) { return bf16_lo(r); }
+  __device__ __forceinline__ static float hi(Entry r) { return bf16_hi(r); }
+};
+struct TabInt8x2 {   // HRF_TABLE_INT8X2: symmetric int8 codes, the slice scales folded into the vectors (quantize.cu)
+  using Entry = uint16_t;
+  __device__ __forceinline__ static float lo(Entry r) { return (float)(int)(int8_t)(r & 0xffu); }
+  __device__ __forceinline__ static float hi(Entry r) { return (float)(int)(int8_t)(r >> 8); }
+};
+
+// Trilinear gather of one level of one grid -> 2 features (fp32 blend of the entries, in corner order).
+template <class Fmt = TabBf16x2>
+__device__ __forceinline__ float2 gather_level(const typename Fmt::Entry* __restrict__ tab, bool hashed, uint32_t res,
                                                uint32_t size, Cell a, Cell b, Cell c) {
-  uint32_t idx[8], raw[8];
+  uint32_t idx[8];
+  typename Fmt::Entry raw[8];
   float w[8];
   corner_indices(hashed, res, size, a, b, c, idx);
 #pragma unroll
@@ -206,8 +220,8 @@ __device__ __forceinline__ float2 gather_level(const uint32_t* __restrict__ tab,
   float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    acc.x = __fmaf_rn(w[k], bf16_lo(raw[k]), acc.x);
-    acc.y = __fmaf_rn(w[k], bf16_hi(raw[k]), acc.y);
+    acc.x = __fmaf_rn(w[k], Fmt::lo(raw[k]), acc.x);
+    acc.y = __fmaf_rn(w[k], Fmt::hi(raw[k]), acc.y);
   }
   return acc;
 }
@@ -318,7 +332,9 @@ __device__ __forceinline__ void write_color_input(const hrf_field& f, unsigned c
 // to gather the tables a second time.
 // kLevelUnroll = 4 keeps four levels' gathers in flight per thread; 2 / 1 shrink the unrolled code.  The forward kernel
 // runs fastest with 1 (it was instruction-cache bound at 4: 117 KB of SASS), see launch_field_forward.
-template <bool kSaveGrid = false, int kLevelUnroll = 4>
+// Fmt: the table entry format (TabInt8x2 for a field with table_format HRF_TABLE_INT8X2; the composition is the same,
+// the folded vectors carry the scales).
+template <bool kSaveGrid = false, int kLevelUnroll = 4, class Fmt = TabBf16x2>
 __device__ __forceinline__ void encode_to_smem(const hrf_field& f, const Sample& s, unsigned char* abuf, int row,
                                                uint32_t* egrid = nullptr, int64_t i = 0, int64_t n = 0) {
   const uint32_t roff = a_row_off(row);
@@ -328,10 +344,11 @@ __device__ __forceinline__ void encode_to_smem(const hrf_field& f, const Sample&
     return;
   }
   const hrf_segment* sg = s.seg;
-  const uint32_t* g0 = sg->grid[0];
-  const uint32_t* g1 = sg->grid[1];
-  const uint32_t* g2 = sg->grid[2];
-  const uint32_t* g3 = sg->grid[3];
+  using Entry = typename Fmt::Entry;
+  const Entry* g0 = reinterpret_cast<const Entry*>(sg->grid[0]);
+  const Entry* g1 = reinterpret_cast<const Entry*>(sg->grid[1]);
+  const Entry* g2 = reinterpret_cast<const Entry*>(sg->grid[2]);
+  const Entry* g3 = reinterpret_cast<const Entry*>(sg->grid[3]);
   const uint32_t hmask = sg->hashed_mask;
   const RowTap2 tx = make_row_tap2(s.x, f.vec_res), ty = make_row_tap2(s.y, f.vec_res), tz = make_row_tap2(s.z, f.vec_res),
                 tt = make_row_tap2(s.t, f.vec_res);
@@ -348,10 +365,10 @@ __device__ __forceinline__ void encode_to_smem(const hrf_field& f, const Sample&
     const bool hashed = (hmask >> l) & 1u;
     const Cell cx = to_cell(scale, s.x), cy = to_cell(scale, s.y), cz = to_cell(scale, s.z), ct = to_cell(scale, s.t);
     // decomposition4d.py:126-129 : xyz, xyt, yzt, xzt
-    const float2 e0 = gather_level(g0 + off, hashed, res, size, cx, cy, cz);
-    const float2 e1 = gather_level(g1 + off, hashed, res, size, cx, cy, ct);
-    const float2 e2 = gather_level(g2 + off, hashed, res, size, cy, cz, ct);
-    const float2 e3 = gather_level(g3 + off, hashed, res, size, cx, cz, ct);
+    const float2 e0 = gather_level<Fmt>(g0 + off, hashed, res, size, cx, cy, cz);
+    const float2 e1 = gather_level<Fmt>(g1 + off, hashed, res, size, cx, cy, ct);
+    const float2 e2 = gather_level<Fmt>(g2 + off, hashed, res, size, cy, cz, ct);
+    const float2 e3 = gather_level<Fmt>(g3 + off, hashed, res, size, cx, cz, ct);
     const float* vl = vbase + (uint32_t)l * vlevel;
     const float2 vx = lerp_row_tap(vl, vstride, tx), vy = lerp_row_tap(vl + vaxis, vstride, ty),
                  vz = lerp_row_tap(vl + 2u * vaxis, vstride, tz), vt_ = lerp_row_tap(vl + 3u * vaxis, vstride, tt);

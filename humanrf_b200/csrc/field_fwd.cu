@@ -30,9 +30,10 @@ __device__ __forceinline__ float warp_sum_fwd(float v) {
 // kDepth (kComposite only): one more scan, of w * t_mid with t_mid = (t + (t + step)) / 2, gives each ray the unnormalised
 // expected distance sum w * t_mid (args.depth; slot 5 of a cut segment's partial).  The other scans are unchanged, so
 // colour and weights sum are bit-identical to those of the kernel without it.
-template <bool kSimt, int kCtasPerSm, bool kSaveGrid = false, int kLevelUnroll = 4, bool kFromFeat = false, bool kComposite = false,
-          bool kDepth = false>
-__global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const __grid_constant__ FieldArgs args) {
+// Fmt: the table entry format (field_common.cuh); the bf16 kernels are field_forward_kernel, the int8 ones
+// field_forward_i8_kernel.
+template <bool kSimt, bool kSaveGrid, int kLevelUnroll, bool kFromFeat, bool kComposite, bool kDepth, class Fmt>
+__device__ __forceinline__ void field_forward_body(const FieldArgs& args) {
   static_assert(kComposite || !kDepth, "the depth scan is part of the compositing epilogue");
   extern __shared__ unsigned char smem_raw[];
   FwdSmem& sm = *reinterpret_cast<FwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
@@ -111,7 +112,7 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
         *reinterpret_cast<uint4*>(sm.a + kg * kAChunk + ro) = row >= 0 ? __ldg(args.feat_in + row * 4 + kg) : make_uint4(0, 0, 0, 0);
     } else {
       const Sample s = load_sample(f, args.s, valid ? i : n, n);
-      encode_to_smem<kSaveGrid, kLevelUnroll>(f, s, sm.a, tid, (kSaveGrid && valid && s.seg != nullptr) ? args.egrid : nullptr, i, n_stride);
+      encode_to_smem<kSaveGrid, kLevelUnroll, Fmt>(f, s, sm.a, tid, (kSaveGrid && valid && s.seg != nullptr) ? args.egrid : nullptr, i, n_stride);
     }
     if (!kFromFeat && args.feat != nullptr && valid) {
       const uint32_t ro = a_row_off(tid);
@@ -237,6 +238,18 @@ __global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const 
   if (!weights_ready) mbar_wait(&sm.bar_w, 0);  // never leave a bulk copy in flight
 }
 
+template <bool kSimt, int kCtasPerSm, bool kSaveGrid = false, int kLevelUnroll = 4, bool kFromFeat = false, bool kComposite = false,
+          bool kDepth = false>
+__global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_kernel(const __grid_constant__ FieldArgs args) {
+  field_forward_body<kSimt, kSaveGrid, kLevelUnroll, kFromFeat, kComposite, kDepth, TabBf16x2>(args);
+}
+
+// HRF_TABLE_INT8X2 fields: inference only (no per-grid features, no SIMT path), one level per encode step.
+template <int kCtasPerSm, bool kComposite = false, bool kDepth = false>
+__global__ void __launch_bounds__(kTile, kCtasPerSm) field_forward_i8_kernel(const __grid_constant__ FieldArgs args) {
+  field_forward_body<false, false, 1, false, kComposite, kDepth, TabInt8x2>(args);
+}
+
 }  // namespace hrf
 
 using namespace hrf;
@@ -253,8 +266,10 @@ static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t s
     return (v == 4 || v == 6) ? v : 5;
   }();
   static const bool ctas_forced = getenv("HRF_FWD_CTAS") != nullptr;
-  // with camera embeddings the blob is 2 KB larger: 5 CTAs would need the 228 KB carve-out (almost no L1) -> use 4
-  const int ctas = (!ctas_forced && a.f.color_in_width == 48) ? 4 : ctas_per_sm;
+  // with camera embeddings the blob is 2 KB larger: 5 CTAs would need the 228 KB carve-out (almost no L1) -> use 4.
+  // An int8 field takes the defaults whatever HRF_FWD_CTAS / HRF_FWD_UNROLL say: only those are instantiated for it.
+  const bool i8 = a.f.table_format == HRF_TABLE_INT8X2;
+  const int ctas = ((!ctas_forced || i8) && a.f.color_in_width == 48) ? 4 : i8 ? 5 : ctas_per_sm;
   const int64_t max_ctas = (int64_t)sm_count() * ctas;
   const int grid = (int)((tiles < max_ctas && !persistent_full) ? tiles : max_ctas);
   auto launch = [&](auto kernel) -> int {
@@ -267,7 +282,12 @@ static int launch_field_forward(const FieldArgs& a, int mlp_impl, cudaStream_t s
   // 1.38 ms per step, 2 and 4 levels 1.40 ms.  Default 1.
   static const int unroll = [] { const char* e = getenv("HRF_FWD_UNROLL"); const int v = e ? atoi(e) : 1; return (v == 2 || v == 4) ? v : 1; }();
   int rc;
-  if (a.comp.ray_offsets != nullptr && a.depth != nullptr && a.feat_in != nullptr)
+  if (i8 && a.feat_in == nullptr) {   // (the kFromFeat kernels read composed features, not tables)
+    if (a.comp.ray_offsets != nullptr && a.depth != nullptr) rc = launch(field_forward_i8_kernel<5, true, true>);
+    else if (a.comp.ray_offsets != nullptr) rc = launch(field_forward_i8_kernel<5, true>);
+    else if (ctas == 4) rc = launch(field_forward_i8_kernel<4>);
+    else rc = launch(field_forward_i8_kernel<5>);
+  } else if (a.comp.ray_offsets != nullptr && a.depth != nullptr && a.feat_in != nullptr)
     rc = launch(field_forward_kernel<false, 5, false, 1, true, true, true>);
   else if (a.comp.ray_offsets != nullptr && a.depth != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, false, true, true>);
   else if (a.comp.ray_offsets != nullptr && a.feat_in != nullptr) rc = launch(field_forward_kernel<false, 5, false, 1, true, true>);
@@ -297,6 +317,7 @@ static int check_field_args(const hrf_field* f, const hrf_samples* s, int mode) 
   HRF_REQUIRE(f->color_in_width == 32 || f->color_in_width == 48, "color_in_width must be 32 or 48");
   HRF_REQUIRE(f->camera_embedding_dim >= 0 && 31 + f->camera_embedding_dim <= f->color_in_width,
               "camera embedding does not fit the colour-net input width");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2 || f->table_format == HRF_TABLE_INT8X2, "unknown table format");
   if (s->num_samples == 0) return 0;
   if (s->ray_origins != nullptr) {
     HRF_REQUIRE(s->ray_directions && s->ray_frame_numbers && s->sample_distances && s->ray_indices,
@@ -311,6 +332,8 @@ static int check_field_args(const hrf_field* f, const hrf_samples* s, int mode) 
 extern "C" int hrf_field_forward(const hrf_field* f, const hrf_samples* s, int mode, int mlp_impl, float* sigma,
                                  void* geo_bf16, float* rgb, void* feat_bf16, void* grid_feat_bf16, void* stream) {
   if (int rc = check_field_args(f, s, mode)) return rc;
+  HRF_REQUIRE(f->table_format != HRF_TABLE_INT8X2 || (grid_feat_bf16 == nullptr && mlp_impl == 0),
+              "an int8 field (compact model) has no per-grid features and no SIMT path: it serves inference only");
   if (s->num_samples == 0) return 0;
   FieldArgs a;
   a.f = *f;
@@ -453,6 +476,8 @@ extern "C" int hrf_field_density_early_stop(const hrf_field* f, const hrf_sample
   HRF_REQUIRE(s->ray_origins != nullptr, "the early-stop density pass needs the ray-batch form");
   HRF_REQUIRE(ray_offsets != nullptr && sigma != nullptr && workspace != nullptr, "null argument");
   HRF_REQUIRE(step > 0.f && stop_depth > 9.2104f, "stop_depth must stay above -ln(1e-4) so the kept set is exact");
+  HRF_REQUIRE(f->table_format != HRF_TABLE_INT8X2 || grid_feat_bf16 == nullptr,
+              "an int8 field (compact model) has no per-grid features: it serves inference only");
   if (s->num_samples == 0 || num_rays == 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   char* ws = reinterpret_cast<char*>(workspace);

@@ -105,8 +105,8 @@ struct LatticeArgs : DensityTileArgs {
 
 // The persistent tile loop: the item count stays on the device, every CTA walks tiles of Item::kItemsPerTile items of
 // kTile / kItemsPerTile rows each.  Only the sigma net is evaluated: its two layers are the first kWCol1 bytes of the
-// blob, whatever the colour net's width.
-template <class Item>
+// blob, whatever the colour net's width.  Fmt: the table entry format (field_common.cuh).
+template <class Item, class Fmt = TabBf16x2>
 __device__ __forceinline__ void density_tile_loop(const Item& args) {
   extern __shared__ unsigned char smem_raw[];
   FwdSmem& sm = *reinterpret_cast<FwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
@@ -141,7 +141,7 @@ __device__ __forceinline__ void density_tile_loop(const Item& args) {
     s.seg = valid ? seg : nullptr;
     s.t = t_local;
     args.position(id, sub, s);
-    encode_to_smem<false, 1>(f, s, sm.a, tid);
+    encode_to_smem<false, 1, Fmt>(f, s, sm.a, tid);
     if (!weights_ready) {
       mbar_wait(&sm.bar_w, 0);
       weights_ready = true;
@@ -161,6 +161,15 @@ __global__ void __launch_bounds__(kTile, kBakeCtasPerSm) occupancy_bake_kernel(c
 
 __global__ void __launch_bounds__(kTile, kBakeCtasPerSm) density_lattice_kernel(const __grid_constant__ LatticeArgs args) {
   density_tile_loop(args);
+}
+
+// The same two for a field with HRF_TABLE_INT8X2 tables.
+__global__ void __launch_bounds__(kTile, kBakeCtasPerSm) occupancy_bake_i8_kernel(const __grid_constant__ BakeArgs args) {
+  density_tile_loop<BakeArgs, TabInt8x2>(args);
+}
+
+__global__ void __launch_bounds__(kTile, kBakeCtasPerSm) density_lattice_i8_kernel(const __grid_constant__ LatticeArgs args) {
+  density_tile_loop<LatticeArgs, TabInt8x2>(args);
 }
 
 // Dynamic shared memory of the tile loop, and its persistent grid: one full wave, capped by the tiles of a full list.
@@ -242,6 +251,7 @@ extern "C" int hrf_bake_occupancy(const hrf_field* f, int32_t frame_number, cons
                                   void* stream) {
   HRF_REQUIRE(f != nullptr && hull_u8 != nullptr && out_u8 != nullptr && workspace != nullptr, "null argument");
   HRF_REQUIRE(f->mlp_blob != nullptr && f->segments != nullptr && f->frame_to_segment != nullptr, "field not initialised");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2 || f->table_format == HRF_TABLE_INT8X2, "unknown table format");
   HRF_REQUIRE(grid_resolution >= 1 && grid_resolution <= 1024, "grid resolution must be in [1, 1024] (int32 voxel ids)");
   HRF_REQUIRE(frame_number >= 0 && frame_number < f->lut_size, "frame number outside the model's frame table");
   HRF_REQUIRE(step > 0.f && alpha_thre > 0.f && alpha_thre < 1.f, "step must be positive and alpha_thre in (0, 1)");
@@ -263,8 +273,9 @@ extern "C" int hrf_bake_occupancy(const hrf_field* f, int32_t frame_number, cons
   a.step = step, a.alpha_thre = alpha_thre;
   a.live = live, a.max_sigma = max_sigma;
   const int smem = density_tile_smem();
-  HRF_CUDA(cudaFuncSetAttribute(occupancy_bake_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  occupancy_bake_kernel<<<density_tile_grid(n, BakeArgs::kItemsPerTile), kTile, smem, st>>>(a);
+  auto* kernel = f->table_format == HRF_TABLE_INT8X2 ? occupancy_bake_i8_kernel : occupancy_bake_kernel;
+  HRF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  kernel<<<density_tile_grid(n, BakeArgs::kItemsPerTile), kTile, smem, st>>>(a);
   HRF_CHECK_LAUNCH();
 
   dilate_and_kernel<<<blocks, 256, 0, st>>>(hull_u8, live, grid_resolution, out_u8);
@@ -282,6 +293,7 @@ extern "C" int hrf_density_lattice(const hrf_field* f, int32_t frame_number, con
                                    float* sigma, void* workspace, void* stream) {
   HRF_REQUIRE(f != nullptr && sigma != nullptr && workspace != nullptr, "null argument");
   HRF_REQUIRE(f->mlp_blob != nullptr && f->segments != nullptr && f->frame_to_segment != nullptr, "field not initialised");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2 || f->table_format == HRF_TABLE_INT8X2, "unknown table format");
   HRF_REQUIRE(grid_resolution >= 1 && grid_resolution <= 1024,
               "grid resolution must be in [1, 1024] ((G+1)^3 int32 vertex ids)");
   HRF_REQUIRE(frame_number >= 0 && frame_number < f->lut_size, "frame number outside the model's frame table");
@@ -302,8 +314,9 @@ extern "C" int hrf_density_lattice(const hrf_field* f, int32_t frame_number, con
   a.frame = frame_number, a.G = grid_resolution;
   a.sigma = sigma;
   const int smem = density_tile_smem();
-  HRF_CUDA(cudaFuncSetAttribute(density_lattice_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  density_lattice_kernel<<<density_tile_grid(n, LatticeArgs::kItemsPerTile), kTile, smem, st>>>(a);
+  auto* kernel = f->table_format == HRF_TABLE_INT8X2 ? density_lattice_i8_kernel : density_lattice_kernel;
+  HRF_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  kernel<<<density_tile_grid(n, LatticeArgs::kItemsPerTile), kTile, smem, st>>>(a);
   HRF_CHECK_LAUNCH();
   return 0;
 }

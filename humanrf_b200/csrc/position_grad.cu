@@ -140,6 +140,7 @@ using namespace hrf;
 extern "C" int hrf_field_position_grad(const hrf_field* f, const hrf_samples* s, const void* workspace, float* d_positions,
                                        void* stream) {
   HRF_REQUIRE(f != nullptr && s != nullptr, "null argument");
+  HRF_REQUIRE(f->table_format == HRF_TABLE_BF16X2, "an int8 field (compact model) serves inference only: it has no gradients");
   HRF_REQUIRE(s->num_samples >= 0, "negative sample count");
   if (s->num_samples == 0) return 0;
   HRF_REQUIRE(workspace != nullptr, "needs the workspace hrf_field_backward_mlp filled");

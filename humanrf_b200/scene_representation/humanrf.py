@@ -82,6 +82,9 @@ class HumanRF(torch.nn.Module):
         self.num_frames = len(sorted_frame_numbers)
         self.sorted_frame_numbers = tuple(int(f) for f in sorted_frame_numbers)
         self.num_segments = len(segment_sizes)
+        self.segment_sizes = tuple(int(s) for s in segment_sizes)
+        self.log2_hashmap_size = int(log2_hashmap_size)
+        self.coarsest_resolution, self.finest_resolution = int(coarsest_resolution), int(finest_resolution)
         self.camera_embedding_dim = camera_embedding_dim
         if camera_embedding_dim > 0:
             self.camera_embeddings = torch.nn.Embedding(160, camera_embedding_dim)  # humanrf.py:75-76
@@ -167,6 +170,10 @@ class HumanRF(torch.nn.Module):
         if self.camera_embedding_dim > 0:
             params.append({'params': self.camera_embeddings.parameters(), 'lr': lr})
         return params
+
+    @property
+    def device(self) -> torch.device:
+        return self.sigma_net.params.device
 
     # ------------------------------------------------------------------ native plumbing
     def hot_parameters(self) -> List[torch.nn.Parameter]:

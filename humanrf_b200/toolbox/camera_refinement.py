@@ -170,6 +170,9 @@ def refine_camera(model, loader, camera_number: int, frame_numbers: Sequence[int
     drawn from `seed`, so a run is deterministic.  Landscape images only (the loader's TEST-mode convention for the
     view's size).  `intrinsics`: also refine the camera's (alpha, beta) (module docstring), with Adam at `intrinsics_lr`
     (default `lr`) on the same schedule; the result then carries the refined focal length and principal point."""
+    from .compact_model import require_trainable
+
+    require_trainable(model, "refine_camera")
     from ..dataset import ray_sampler_native as rs
     from ..dataset.cameras import rotation_from_axisangle
     from ..dataset.input_batch import InputBatch

@@ -330,6 +330,9 @@ class CameraResponses:
         camera and the reason, when a camera cannot be fitted (fewer than `min_pixels` pixels, a singular system, a gain
         <= 0); nothing has been written then.  Fitting a camera again replaces its earlier fit.  Returns a
         ``ResponseFit`` per camera, in camera order; ``fits`` and ``fitted_pairs`` keep them."""
+        from .compact_model import require_trainable
+
+        require_trainable(model, "fit_held_out")
         from .depth_maps import _Views
         from .evaluation import ground_truth
         from .learned_occupancy import bake_occupancy_grid

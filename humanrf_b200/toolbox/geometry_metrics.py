@@ -287,7 +287,7 @@ def evaluate_geometry(model, dataset, frames, reference_dir, out_dir, level: flo
     if missing:
         raise RuntimeError(f"missing reference meshes: {missing}")
     offset, scale = scene_normalisation(dataset)
-    dev = model.sigma_net.params.device
+    dev = model.device
     vals = torch.empty((len(frames), 2, 3), dtype=torch.float64, device=dev)
     cnt = torch.empty((len(frames), 2, len(taus)), dtype=torch.int64, device=dev)
     err = torch.empty((len(frames), 2), dtype=torch.int32, device=dev)

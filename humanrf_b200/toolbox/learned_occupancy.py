@@ -51,7 +51,7 @@ def bake_occupancy_grid(model, frame_number: int, hull: torch.Tensor, render_ste
     if frame not in model.sorted_frame_numbers:
         raise RuntimeError(f"frame {frame} is not one of the model's frames")
     nat = model.native()
-    if hull.device != model.sigma_net.params.device:
+    if hull.device != model.device:
         raise RuntimeError("hull and model must be on the same CUDA device")
     lib = L.lib()
     ws = torch.empty(int(lib.hrf_bake_occupancy_workspace_bytes(G)), dtype=torch.uint8, device=hull.device)
@@ -87,7 +87,7 @@ class LearnedOccupancyDataset:
         frame = int(frame_number)
         grid = self._grids.get(frame)
         if grid is None:
-            device = self.model.sigma_net.params.device
+            device = self.model.device
             hull = torch.from_numpy(np.ascontiguousarray(self.dataset.get_occupancy_grid(frame_number=frame))).to(device)
             grid = bake_occupancy_grid(self.model, frame, hull, self.render_step_size).cpu().numpy()
             self._grids[frame] = grid

@@ -59,7 +59,7 @@ def density_lattice(model, frame_number: int, mask: Optional[torch.Tensor] = Non
     G is the mask's and only the corners of occupied voxels are evaluated (0 elsewhere); without one, `resolution` is
     G and every vertex is evaluated.  Each value is exactly ``model.density`` (query form) at that position."""
     frame = _check_frame(model, frame_number)
-    device = model.sigma_net.params.device
+    device = model.device
     if mask is not None:
         G = _check_grid(mask, "mask")
         if resolution is not None and int(resolution) != G:
@@ -202,7 +202,7 @@ def export_mesh_sequence(model, dataset, frames, out_dir, level: float, bake: bo
 
     frames = [_check_frame(model, f) for f in frames]
     offset, scale = scene_normalisation(dataset)
-    device = model.sigma_net.params.device
+    device = model.device
     os.makedirs(out_dir, exist_ok=True)
     paths = []
     for frame in frames:

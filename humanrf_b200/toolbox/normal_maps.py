@@ -17,6 +17,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from .compact_model import require_trainable
 from .depth_maps import _check_camera, _check_frame, _Views, camera_name, write_depth_exr
 
 
@@ -50,6 +51,7 @@ def render_normal_map(model, loader, camera_number: int, frame_number: int, grid
                       render_step_size: float = 4e-4, rays_per_batch: int = 262144) -> NormalMap:
     """Alpha and normal maps of `model` seen from `loader`'s camera `camera_number` at `frame_number` (the view and
     `grid` as for ``render_depth_map``: the frame's hull by default, or a given uint8 [G,G,G] grid)."""
+    require_trainable(model, "normal maps (they need the density's position gradient)")
     frame = _check_frame(model, frame_number)
     c = _check_camera(loader, camera_number)
     views = _Views(model, loader, render_step_size, rays_per_batch)
@@ -73,6 +75,7 @@ def export_normal_sequence(model, loader, pairs, out_dir, bake: bool = True, ren
     (<cam> = ``camera_name``): ``render_normal_map``'s camera-frame normals, float32, x, y, z in R, G, B, 0 on
     background.  With `bake`, each frame's hull is tightened by ``bake_occupancy_grid`` first (once per frame).
     Cameras and frames are checked before anything is written.  Returns the written paths."""
+    require_trainable(model, "normal maps (they need the density's position gradient)")
     from .learned_occupancy import bake_occupancy_grid
 
     pairs = [(_check_camera(loader, c), _check_frame(model, f)) for c, f in pairs]

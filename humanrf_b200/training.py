@@ -81,6 +81,9 @@ class FusedTrainer:
         camera_responses: a toolbox.camera_response.CameraResponses over the same loader; each camera's colour response
         is refined with the field (then step() needs `cameras`).  The same world_size, process_group and
         overlap_exchange rules as camera_poses."""
+        from .toolbox.compact_model import require_trainable
+
+        require_trainable(model, "FusedTrainer")
         for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses)):
             if calib is None:
                 continue

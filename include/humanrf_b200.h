@@ -127,7 +127,15 @@ typedef struct {
   const float* camera_embeddings;
   int32_t  camera_embedding_dim, num_cameras;
   int32_t  color_in_width;           /* 32 (no embedding) or 48: width of the padded colour-net input */
+  /* HRF_TABLE_BF16X2: hrf_segment.grid[k] holds bf16x2 entries (uint32_t each).
+   * HRF_TABLE_INT8X2: it holds int8x2 entries (uint16_t each: feature 0 in the low byte) with the same entry indexing,
+   * and `vectors` / `vectors_t` carry each slice's scale folded in (hrf_quantize_tables_write).  Only inference reads
+   * such a field: every backward entry, hrf_field_position_grad, a forward asking for the per-grid features and the
+   * SIMT debug path (mlp_impl != 0) refuse it, because the per-grid features are no longer the model's. */
+  int32_t  table_format;
 } hrf_field;
+#define HRF_TABLE_BF16X2 0
+#define HRF_TABLE_INT8X2 1
 
 /* Sample source: either explicit per-sample queries (QueryInput, query_io.py:6-13) or the
  * ray-batch form used by prune_samples/render (volume_rendering.py:66-72,110-119). */
@@ -414,6 +422,26 @@ int hrf_adam_step(float* param, float* exp_avg, float* exp_avg_sq, const float* 
 int hrf_cast_bf16(const float* src, void* dst_bf16, int64_t n, void* stream);
 /* vectors [4, vec_res, 32] -> vectors_t [4, 16, vec_res, 2] (hrf_segment.vectors_t) */
 int hrf_transpose_vectors(const float* vectors, float* vectors_t, int vec_res, void* stream);
+
+/* 8-bit tables for inference (HRF_TABLE_INT8X2, DESIGN.md §3.19), from the fp32 masters of one segment.  masters: host
+ * array of the 4 grids' device tables [n_entries, 2] (tcnn layout), level_offset / level_size: host [16].  A slice is one
+ * (grid, level, feature); its scale s and codes q follow, with every rounding pinned:
+ *   s = (c * absmax) / 127 (two fp32 roundings), q = s == 0 ? 0 : clamp(rint(x / s), -127, 127)
+ * with the clip ratio c taken from the fixed list {1, 0.9, ..., 0.3} that minimises sum (x - s q)^2 over the slice
+ * (float64; ties go to the larger c).
+ * Pass one: scale / clip (index into the list) [4][16][2] and sq_err [4][16][2][8] (float64, per candidate), all device;
+ * status is device scratch [4][16].  It reads the stream's result back: a non-finite master value fails, naming the
+ * segment (`segment`, for the message), grid and level, and nothing else is to be used then. */
+#define HRF_QUANT_CLIPS 8
+int hrf_quantize_tables_select(const float* const* masters, const uint32_t* level_offset, const uint32_t* level_size,
+                               int segment, float* scale, int32_t* clip, double* sq_err, int32_t* status, void* stream);
+/* Pass two: the codes of the 4 grids, int8x2 [n_entries] each (codes: host array of 4 device pointers). */
+int hrf_quantize_tables_write(const float* const* masters, const uint32_t* level_offset, const uint32_t* level_size,
+                              const float* scale /* device [4][16][2] */, void* const* codes, void* stream);
+/* The scales folded into the vectors: folded[a][row][2l+f] = s(grid(a), l, f) * vectors[a][row][2l+f], the grid composed
+ * with axis a being yzt, xzt, xyt, xyz for a = x, y, z, t.  Then hrf_transpose_vectors(folded) gives vectors_t. */
+int hrf_quantize_fold_vectors(const float* vectors, const float* scale /* device [4][16][2] */, int vec_res, float* folded,
+                              void* stream);
 
 /* All parameter tensors of a model in ONE launch (the per-tensor entry point above costs one launch per tensor: 23
  * for a single segment).  tensors: device array of descriptors; a tensor whose *active flag is 0 is skipped entirely
