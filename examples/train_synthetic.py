@@ -85,13 +85,17 @@ def psnr(a, b):
     return float(-10 * torch.log10(torch.mean((a - b) ** 2)))      # trainer.py:218-222
 
 
-def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet=False, return_state=False):
+def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet=False, return_state=False, seed=0,
+         error_map=None, sample_budget=None):
     """Returns the held-out PSNR history [(step, dB)]; with `return_state` also a dict of the trained student, the
-    dataset, the occupancy grid, the camera-table builder, the frames and the held-out camera."""
+    dataset, the occupancy grid, the camera-table builder, the frames, the held-out camera and the samples trained on.
+    `seed` seeds the run (the student, the pair schedule, the trainer's jitter and backgrounds; the teacher and the scene
+    stay).  `error_map`: keyword arguments of toolbox.error_map.ErrorMap, whose seed is `seed`: the rays are drawn from
+    it.  `sample_budget`: stop once the steps have trained on that many samples (`steps` stays the limit)."""
     from humanrf_b200.dataset.occupancy_grid_native import OccupanyGrid
 
     dev = torch.device("cuda:0")
-    torch.manual_seed(0); np.random.seed(0)
+    torch.manual_seed(seed); np.random.seed(seed)
     frames = list(range(15, 21))
     teacher = smooth_teacher(dev, frames)
     ds = TeacherDataset(teacher, dev, num_cameras=6, frames=frames, width=96, height=72, G=64)
@@ -108,8 +112,13 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
     dl = DataLoader(ds, "cuda", M.TRAINING, DataLoader.OutputMode.RAYS_AND_SAMPLES, DataLoader.SpacePruningMode.OCCUPANCY_GRID,
                     batch_size=rays_initial, camera_numbers=train_cams, frame_numbers=tuple(frames), max_buffer_size=64,
                     max_num_frames_per_batch=8, use_mask=True, filter_light_bloom=False)
-    student, _ = make_model((len(frames),), first_frame=frames[0], seed=1, table_std=1e-4, device=dev)
-    trainer = FusedTrainer(student, lr=1e-2, max_steps=steps, prune=False)
+    student, _ = make_model((len(frames),), first_frame=frames[0], seed=1 + seed, table_std=1e-4, device=dev)
+    emap = None
+    if error_map is not None:
+        from humanrf_b200.toolbox.error_map import ErrorMap
+
+        emap = ErrorMap(dl, seed=seed, **error_map)
+    trainer = FusedTrainer(student, lr=1e-2, max_steps=steps, prune=False, seed=123 + seed, error_map=emap)
     renderer = TileShardedRenderer(student, og, rays_per_batch=8192)
 
     def validate():
@@ -124,13 +133,15 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
     history = [(0, validate())]
     it = iter(dl)
     t0 = time.time()
-    rays_done = 0
+    rays_done = samples_done = 0
     for step in range(1, steps + 1):
         dl.batch_size = rays_initial                                             # trainer.py:139
         total_rays = total_samples = 0
-        batches = []
+        batches, pixels = [], []
         while True:                                                              # trainer.py:143-163
             b = next(it)
+            if emap is not None:                                                 # the pool index of each kept ray
+                pixels.append(dl.last_ray_indices[b.ray_masks.view(-1)])
             prune_samples(b, student, is_training=True)
             batches.append(b)
             total_rays += dl.batch_size
@@ -143,17 +154,23 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
         ib = merge_input_batches(batches, max_num_samples=int(samples_max * 1.1))   # trainer.py:170-172
         if ib.num_samples == 0:
             continue
+        px = torch.cat(pixels)[:ib.num_rays] if emap is not None else None     # merging keeps a prefix of the rays
         trainer.step(ib.ray_origins.contiguous(), ib.ray_directions.contiguous(), ib.frame_numbers.view(-1).contiguous(),
-                     ib.sample_distances.view(-1).contiguous(), ib.ray_indices.contiguous(), ib.rgba.contiguous(), ib.num_rays)
+                     ib.sample_distances.view(-1).contiguous(), ib.ray_indices.contiguous(), ib.rgba.contiguous(), ib.num_rays,
+                     pixels=px)
         rays_done += ib.num_rays
-        if step % log_every == 0 or step == steps:
+        samples_done += ib.num_samples
+        last = step == steps or (sample_budget is not None and samples_done >= sample_budget)
+        if step % log_every == 0 or last:
             history.append((step, validate()))
             if not quiet:
                 print(f"step {step:5d}  loss {float(trainer.last['loss']):.5f}  samples {ib.num_samples}  rays {ib.num_rays}  "
                       f"held-out PSNR {history[-1][1]:.2f} dB  ({rays_done / (time.time() - t0):.0f} rays/s incl. validation)")
+        if last:
+            break
     if return_state:
         return history, dict(student=student, dataset=ds, occupancy_grid=og, tables=tables, frames=frames,
-                             held_out=held_out)
+                             held_out=held_out, samples=samples_done, steps=step)
     return history
 
 

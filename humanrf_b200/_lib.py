@@ -75,6 +75,10 @@ class CameraIntrinsics(C.Structure):
                 ("base_rotations", vp), ("rotations", vp)]
 
 
+class ErrorMapGeometry(C.Structure):
+    _fields_ = [("landscape_modes", vp), ("num_slots", i64), ("image_width", i32), ("image_height", i32), ("tile", i32)]
+
+
 ADAM_BLOCK_ELEMS = 4096
 DP_MAX_WORLD = 8
 
@@ -163,6 +167,13 @@ _SIGNATURES = {
     "hrf_response_fit_accumulate": (C.c_int, [vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp]),
     "hrf_response_fit_solve": (C.c_int, [C.POINTER(CameraResponses), vp, vp, C.c_int, C.c_double, C.c_double, vp, vp,
                                          vp]),
+    "hrf_error_map_num_tiles": (i64, [C.POINTER(ErrorMapGeometry), f32]),
+    "hrf_error_map_workspace_bytes": (i64, [i64]),
+    "hrf_error_map_accumulate": (C.c_int, [vp, vp, vp, vp, vp, i64, vp, vp, C.c_int, f32, C.POINTER(ErrorMapGeometry),
+                                           vp, vp, vp, vp]),
+    "hrf_error_map_update": (C.c_int, [C.POINTER(ErrorMapGeometry), vp, vp, vp, f32, f32, vp, vp, vp]),
+    "hrf_error_map_draw": (C.c_int, [vp, C.POINTER(ErrorMapGeometry), u64, u64, i64, C.c_double, vp, vp]),
+    "hrf_error_map_reset_slots": (C.c_int, [C.POINTER(ErrorMapGeometry), i64, i64, f32, vp, vp]),
     "hrf_compose_tensors_forward": (C.c_int, [vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_backward": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),

@@ -46,16 +46,6 @@ __host__ __device__ inline int response_blocks(int64_t num_rays) {
   return (int)(b < kRespMaxBlocks ? b : kRespMaxBlocks);
 }
 
-// The response of one channel: color + em (color - (1 - w) bg) + w b, with a zero em or b not added (so that em = b = 0
-// returns color bit for bit).  The loss kernel and hrf_camera_response_apply share it.
-__device__ __forceinline__ float respond(float color, float w, float bg, float em, float b, float& fg) {
-  fg = __fmaf_rn(-(1.f - w), bg, color);
-  float pred = color;
-  if (em != 0.f) pred = __fmaf_rn(em, fg, pred);
-  if (b != 0.f) pred = __fmaf_rn(w, b, pred);
-  return pred;
-}
-
 __global__ void __launch_bounds__(kRespThreads) response_loss_kernel(
     const float* __restrict__ color, const float* __restrict__ wsum, const float* __restrict__ rgba,
     const float* __restrict__ bg, const int32_t* __restrict__ camera_numbers, const float* __restrict__ table,

@@ -134,6 +134,7 @@ class DataLoader:
             self.cuda_grid_texture = occupancy_grid_native.OccupanyGrid(self.occupancy_grid_resolution,
                                                                         self.occupancy_grids_buffer_size)
         self.replacing = False
+        self.ray_source = None             # TRAINING: an object whose draw(batch_size) replaces torch.randint (ErrorMap)
         self.slot_pairs = [None] * self.buffer_size           # the (camera, frame) pair every pool slot currently holds
         self.camera_frame_pairs = self._camera_frame_pair_generator()
         for slot in range(self.buffer_size):
@@ -210,6 +211,8 @@ class DataLoader:
         self.landscape_mode_cuda[buffer_index] = camera.width > camera.height
         self.inverse_krs_cuda[buffer_index].copy_(self.all_inverse_krs[camera_number])
         self.camera_origins_cuda[buffer_index].copy_(self.all_camera_origins[camera_number])
+        if self.ray_source is not None:
+            self.ray_source.reset_slot(buffer_index)
 
     # ------------------------------------------------------------------------------------------------
     @property
@@ -240,8 +243,11 @@ class DataLoader:
                 for _ in range(self.replace_per_next):        # what the reference's replacer thread does in the background
                     self._load_and_copy_camera_frame_data(next(self.camera_frame_pairs), self.pair_load_index % self.buffer_size)
                     self.pair_load_index += 1
-            ray_indices = torch.randint(0, self.buffer_size * self.num_pixels_per_camera, size=(self.batch_size,),
-                                        dtype=torch.int64, device=self.device)
+            if self.ray_source is not None:
+                ray_indices = self.ray_source.draw(self.batch_size)
+            else:
+                ray_indices = torch.randint(0, self.buffer_size * self.num_pixels_per_camera, size=(self.batch_size,),
+                                            dtype=torch.int64, device=self.device)
             out = self.ray_sampler_func(self.pixel_colors.view(-1, 4), self.light_mask.view(-1), self.frame_numbers_cuda,
                                         self.camera_numbers_cuda, self.grid_texture_objects_cuda, self.landscape_mode_cuda,
                                         ray_indices, self.inverse_krs_cuda, self.camera_origins_cuda, self.aabb,

@@ -38,6 +38,11 @@ start step on, the loss runs through each ray's camera response (hrf_train_loss_
 gradient per camera), and after the field's Adam, where the pose step runs, the per-camera Adam on the responses
 (hrf_camera_response_step).  Data parallel: their gradient record travels as the pose record does.  Without
 camera_responses, or before their start step, the step launches exactly the kernels it launches without them.
+
+Error map (`error_map=`, toolbox/error_map.py ErrorMap, DESIGN.md §3.20): right after the loss kernel, on the step's
+stream, the step adds each ray's colour Huber error into its pool pixel's tile (hrf_error_map_accumulate, fed by the
+batch's pool indices `pixels`) and folds the tiles into the map (hrf_error_map_update); the loader's next draw reads it.
+Both only read the step's buffers: the field's update is the one the step makes without an error map.
 """
 from __future__ import annotations
 
@@ -72,7 +77,7 @@ class FusedTrainer:
                  max_steps: int = 50001, bce_loss_weight: float = 1e-3, huber_delta: float = 0.01,
                  render_step_size: float = 4e-4, world_size: int = 1, process_group=None, prune: bool = True,
                  seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False,
-                 camera_poses=None, camera_responses=None):
+                 camera_poses=None, camera_responses=None, error_map=None):
         """camera_poses: a toolbox.camera_refinement.CameraPoses over the loader the batches come from; its cameras'
         poses are refined with the field (then step() needs `cameras`).  Its world_size must be this trainer's: with
         world_size > 1 every rank builds its own CameraPoses over its own loader, the ranks exchange their per-camera
@@ -80,7 +85,9 @@ class FusedTrainer:
         take camera_poses with world_size > 1 (ValueError).
         camera_responses: a toolbox.camera_response.CameraResponses over the same loader; each camera's colour response
         is refined with the field (then step() needs `cameras`).  The same world_size, process_group and
-        overlap_exchange rules as camera_poses."""
+        overlap_exchange rules as camera_poses.
+        error_map: a toolbox.error_map.ErrorMap over the loader the batches come from (then step() needs `pixels`); with
+        world_size > 1 every rank has its own, built with its rank."""
         from .toolbox.compact_model import require_trainable
 
         require_trainable(model, "FusedTrainer")
@@ -109,9 +116,11 @@ class FusedTrainer:
         # more than one: off by default.
         self.overlap_exchange = bool(overlap_exchange) and self.exchange == "p2p"
         self.rank = dist.get_rank(process_group) if world_size > 1 else 0
-        for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses)):
+        for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses),
+                            ("error_map", error_map)):
             if calib is not None and calib.rank != self.rank:
                 raise ValueError(f"{name} has rank {calib.rank}, the trainer rank {self.rank}")
+        self.error_map = error_map
         self.params: List[torch.nn.Parameter] = model.hot_parameters()
         dev = self.params[0].device
         self.dev = dev
@@ -303,12 +312,15 @@ class FusedTrainer:
         return self.lr * self.lr_decay ** min(self.t / self.max_steps, 1.0)
 
     def step(self, o, d, frames, t, ri, rgba, num_rays: int, kernel_event=None, return_loss: bool = False,
-             background: Optional[torch.Tensor] = None, cameras: Optional[torch.Tensor] = None, bwd_events=None):
+             background: Optional[torch.Tensor] = None, cameras: Optional[torch.Tensor] = None, bwd_events=None,
+             pixels: Optional[torch.Tensor] = None):
         """One optimisation step on a ray batch given in InputBatch layout (device tensors; `ri` int64 as in the reference's
         InputBatch.ray_indices, or int32).  Nothing in here reads
         the device back: the step is enqueued and the call returns.  Returns the number of kernels launched, or the
         loss value when return_loss (that one read is the caller's choice).  With camera_poses, from its start step on,
-        `cameras` (int32 [R], the camera of each ray) is required and the poses take one Adam step too."""
+        `cameras` (int32 [R], the camera of each ray) is required and the poses take one Adam step too.  With an
+        error_map, `pixels` (int64 [R], the batch's pool indices: the loader's last_ray_indices of that batch) is
+        required."""
         lib, nat, dev = L.lib(), self.model.native(), t.device
         launches = 0
         poses = self.camera_poses if (self.camera_poses is not None and self.camera_poses.active(self.t)) else None
@@ -321,6 +333,12 @@ class FusedTrainer:
             cameras = L.require_cuda(cameras.reshape(-1), "cameras", torch.int32)
             if cameras.numel() != num_rays:
                 raise ValueError(f"cameras holds {cameras.numel()} entries for {num_rays} rays")
+        if self.error_map is not None:
+            if pixels is None:
+                raise ValueError("error_map: step() needs the pool index of every ray (`pixels`, int64 [R])")
+            pixels = L.require_cuda(pixels.reshape(-1), "pixels", torch.int64)
+            if pixels.numel() != num_rays:
+                raise ValueError(f"pixels holds {pixels.numel()} entries for {num_rays} rays")
         t_done = self.t
         marks = [] if self.profile else None
 
@@ -419,6 +437,11 @@ class FusedTrainer:
         else:
             launches += resp.loss(color, wsum, rgba, bg, cameras, num_rays, self.delta, self.bce_w, loss_scale, d_color,
                                   d_wsum, loss) - 1
+        if self.error_map is not None:
+            launches += self.error_map.accumulate(color, wsum, rgba, bg, pixels, num_rays, self.delta,
+                                                  None if resp is None else resp.table,
+                                                  None if resp is None else cameras)
+            launches += self.error_map.update()
         # ---- backward: compositing, then the fused field backward into the flat bucket (clean: Adam re-zeroes it)
         d_sigma = torch.empty(n_cap, dtype=torch.float32, device=dev)
         d_rgb = torch.empty((n_cap, 3), dtype=torch.float32, device=dev)

@@ -869,6 +869,62 @@ int hrf_depth_metrics(const float* pred_z, const uint8_t* pred_mask, const float
                       int32_t* error /* [1] device */, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Error map of the training pool (toolbox/error_map.py ErrorMap, DESIGN.md §3.20): a running per-tile colour error of
+ * every pooled image, fed by the fused train step, from which the loader draws the next batch's pool indices.
+ * Pool pixel slot * P + p (P = W H).  Its (x, y) is the sampler's: a slot with landscape_modes[slot] != 0 is W wide and
+ * H high, any other slot H wide and W high; x = p % width, y = p / width.  Tiles are T x T pixels in the slot's own
+ * orientation, row-major, ceil(width / T) per row: every slot has ceil(W/T) ceil(H/T) tiles, tile t of slot s is global
+ * tile s * tiles_per_slot + t, and a border tile holds npix = min(T, width - x0) min(T, height - y0) pixels.
+ * Every entry is asynchronous on `stream` and reads nothing back to the host.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  const uint8_t* landscape_modes;     /* [B] device: the loader's landscape_mode_cuda */
+  int64_t num_slots;                  /* B */
+  int32_t image_width;                /* W, as the sampler takes it */
+  int32_t image_height;               /* H */
+  int32_t tile;                       /* T, 1..4096 */
+} hrf_error_map_geometry;
+/* B ceil(W/T) ceil(H/T), or -1 for a bad geometry or one where the total weight could reach 2^63 with every EMA and the
+ * floor at most max(max_ema, 1) (pass max(prior, floor): the EMA of values below 1 started at the prior never exceeds
+ * max(prior, 1)). */
+int64_t hrf_error_map_num_tiles(const hrf_error_map_geometry* geometry, float max_ema);
+int64_t hrf_error_map_workspace_bytes(int64_t num_tiles);          /* 8 ceil(tiles / 2048), -1 for tiles < 1 */
+/* One launch.  Per ray, e_r = h_0 + h_1 + h_2 (fp32, in channel order) with h_k hrf_train_loss's Huber value of
+ * channel k before its 1 / (3R) and loss_scale, rounded as that kernel is compiled: gt = fma(m, rgb_k, (1 - m) bg_k),
+ * x = color_k - gt, h = (x / 2) x when |x| < delta, else (|x| - delta / 2) delta.  With response_table (then
+ * camera_numbers and weights_sum too) it is hrf_train_loss_response's value as that kernel is compiled: color_k is first
+ * taken through the ray's camera response (a camera outside [0, num_cameras) takes the identity), and
+ * gt = fma(1 - m, bg_k, m rgb_k).  q_r = min(rint(e_r 2^32),
+ * 2^32 - 1) (NaN: the cap) is added into tile_sum of the ray's tile and tile_count += 1 (integer atomics: the result
+ * does not depend on scheduling).  A pixel outside [0, B P) sets bit 0 of error[0] and the ray is skipped. */
+int hrf_error_map_accumulate(const float* color /* [R,3] */, const float* weights_sum /* [R] or NULL */,
+                             const float* rgba /* [R,4] */, const float* background /* [R,3] */,
+                             const int64_t* pixels /* [R] pool indices */, int64_t num_rays,
+                             const float* response_table /* [C,6] or NULL */, const int32_t* camera_numbers /* [R] */,
+                             int num_cameras, float huber_delta, const hrf_error_map_geometry* geometry,
+                             uint64_t* tile_sum /* [tiles] */, uint32_t* tile_count /* [tiles] */,
+                             int32_t* error /* [1] */, void* stream);
+/* Three launches.  Every tile with count > 0: m = (float)((double)sum / count 2^-32), ema = fma(beta, m - ema, ema),
+ * sum = count = 0; other tiles keep their ema.  Then w_t = rint(max(ema_t, floor) npix_t 2^24) (exact in double) and
+ * cdf = the inclusive scan of w over all tiles (integer, exact).  beta in (0, 1], floor >= 2^-24 (every w_t >= 1), and a
+ * floor for which hrf_error_map_num_tiles(geometry, floor) >= 0.
+ * workspace: hrf_error_map_workspace_bytes(tiles) bytes. */
+int hrf_error_map_update(const hrf_error_map_geometry* geometry, float* ema /* [tiles] */,
+                         uint64_t* tile_sum /* [tiles] */, uint32_t* tile_count /* [tiles] */, float beta,
+                         float floor_weight, uint64_t* cdf /* [tiles] */, void* workspace, void* stream);
+/* One launch.  With key = s(s(seed) ^ counter), s(x) the SplitMix64 finaliser of x + 0x9E3779B97F4A7C15, and
+ * h(r, k) = s(key ^ (4 r + k)): rays r < floor(uniform_fraction R) take out[r] = umulhi(h(r, 0), B P); every other ray
+ * takes tile t = upper_bound(cdf, umulhi(h(r, 0), cdf[tiles - 1])) (the first tile whose CDF exceeds it) and pixel
+ * k = umulhi(h(r, 1), npix_t) of that tile, row-major inside it. */
+int hrf_error_map_draw(const uint64_t* cdf /* [tiles] */, const hrf_error_map_geometry* geometry, uint64_t seed,
+                       uint64_t counter, int64_t num_rays, double uniform_fraction, int64_t* out /* [R] */,
+                       void* stream);
+/* ema = prior on every tile of slots [first_slot, first_slot + num_slots), one launch over those tiles only.  The CDF
+ * (and so the draw) changes at the next update. */
+int hrf_error_map_reset_slots(const hrf_error_map_geometry* geometry, int64_t first_slot, int64_t num_slots,
+                              float prior, float* ema /* [tiles] */, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
