@@ -86,12 +86,16 @@ def psnr(a, b):
 
 
 def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet=False, return_state=False, seed=0,
-         error_map=None, sample_budget=None):
+         error_map=None, sample_budget=None, training_occupancy=None, loose_hull=False):
     """Returns the held-out PSNR history [(step, dB)]; with `return_state` also a dict of the trained student, the
     dataset, the occupancy grid, the camera-table builder, the frames, the held-out camera and the samples trained on.
     `seed` seeds the run (the student, the pair schedule, the trainer's jitter and backgrounds; the teacher and the scene
     stay).  `error_map`: keyword arguments of toolbox.error_map.ErrorMap, whose seed is `seed`: the rays are drawn from
-    it.  `sample_budget`: stop once the steps have trained on that many samples (`steps` stays the limit)."""
+    it.  `sample_budget`: stop once the steps have trained on that many samples (`steps` stays the limit).
+    `training_occupancy`: keyword arguments of toolbox.training_occupancy.TrainingOccupancy, whose seed is `seed`: the
+    training sampler's grids are learned while training.  `loose_hull`: the images are rendered through the dataset's
+    hulls, then every hull is dilated by 6 voxels for training and validation, so the scene's density sits well inside
+    hulls with slack around it (as around a body seen by few cameras)."""
     from humanrf_b200.dataset.occupancy_grid_native import OccupanyGrid
 
     dev = torch.device("cuda:0")
@@ -108,6 +112,12 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
     og = OccupanyGrid(64, 2)
     tables = camera_tables(boot, og, ds)
     ds.bake(tables, og)
+    if loose_hull:
+        with torch.no_grad():
+            for f in frames:
+                g = torch.from_numpy(ds._grids[f]).to(dev).float()[None, None]
+                ds._grids[f] = (torch.nn.functional.max_pool3d(g, 13, stride=1, padding=6)[0, 0] > 0).to(
+                    torch.uint8).mul(255).cpu().numpy()
     train_cams, held_out = (0, 1, 2, 3, 4), 5
     dl = DataLoader(ds, "cuda", M.TRAINING, DataLoader.OutputMode.RAYS_AND_SAMPLES, DataLoader.SpacePruningMode.OCCUPANCY_GRID,
                     batch_size=rays_initial, camera_numbers=train_cams, frame_numbers=tuple(frames), max_buffer_size=64,
@@ -118,7 +128,13 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
         from humanrf_b200.toolbox.error_map import ErrorMap
 
         emap = ErrorMap(dl, seed=seed, **error_map)
-    trainer = FusedTrainer(student, lr=1e-2, max_steps=steps, prune=False, seed=123 + seed, error_map=emap)
+    tocc = None
+    if training_occupancy is not None:
+        from humanrf_b200.toolbox.training_occupancy import TrainingOccupancy
+
+        tocc = TrainingOccupancy(dl, student, seed=seed, **training_occupancy)
+    trainer = FusedTrainer(student, lr=1e-2, max_steps=steps, prune=False, seed=123 + seed, error_map=emap,
+                           training_occupancy=tocc)
     renderer = TileShardedRenderer(student, og, rays_per_batch=8192)
 
     def validate():
@@ -170,7 +186,7 @@ def main(steps=300, samples_max=200_000, rays_initial=4096, log_every=100, quiet
             break
     if return_state:
         return history, dict(student=student, dataset=ds, occupancy_grid=og, tables=tables, frames=frames,
-                             held_out=held_out, samples=samples_done, steps=step)
+                             held_out=held_out, samples=samples_done, steps=step, loader=dl, training_occupancy=tocc)
     return history
 
 

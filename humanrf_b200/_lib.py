@@ -174,6 +174,12 @@ _SIGNATURES = {
     "hrf_error_map_update": (C.c_int, [C.POINTER(ErrorMapGeometry), vp, vp, vp, f32, f32, vp, vp, vp]),
     "hrf_error_map_draw": (C.c_int, [vp, C.POINTER(ErrorMapGeometry), u64, u64, i64, C.c_double, vp, vp]),
     "hrf_error_map_reset_slots": (C.c_int, [C.POINTER(ErrorMapGeometry), i64, i64, f32, vp, vp]),
+    "hrf_training_occupancy_key": (u64, [u64, i32, u64]),
+    "hrf_training_occupancy_workspace_bytes": (i64, [C.c_int]),
+    "hrf_training_occupancy_compact": (C.c_int, [vp, C.c_int, vp, vp, vp, vp]),
+    "hrf_training_occupancy_update": (C.c_int, [C.POINTER(Field), i32, C.c_int, vp, vp, i64, u64, u64, f32, vp, vp,
+                                                vp]),
+    "hrf_training_occupancy_pack": (C.c_int, [vp, vp, i64, C.c_int, f32, f32, vp, vp, vp, vp]),
     "hrf_compose_tensors_forward": (C.c_int, [vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp]),
     "hrf_compose_tensors_backward": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "hrf_adam_step": (C.c_int, [vp, vp, vp, vp, vp, i64, f32, f32, f32, f32, C.c_int, f32, vp]),

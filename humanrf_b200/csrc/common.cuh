@@ -47,6 +47,23 @@ __device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u 
 __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
+// SplitMix64: the finaliser of x + golden gamma (the counter-based hash of the error map's draws, the mesh sampler and
+// the training occupancy's points).
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+  uint64_t z = x + 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// The bit layout of an occupancy ring slot (hrf_occgrid_add): voxel i is bit i & 31 of word i >> 5, and the bits past
+// the last voxel of the last word are 0.  Called by every lane of a full warp whose lane l holds voxel i0 + l, i0 a
+// multiple of 32; occ is the voxel's occupancy (false for i >= n).
+__device__ __forceinline__ void store_occupancy_bits(uint32_t* __restrict__ bits, int64_t i, int64_t n, bool occ) {
+  const uint32_t b = __ballot_sync(0xffffffffu, occ);
+  if ((threadIdx.x & 31) == 0 && i < n) bits[i >> 5] = b;
+}
+
 // One Adam update of one element (torch.optim.Adam, no weight decay), with every rounding spelled out so that all
 // optimiser kernels and both of their paths (float4 and scalar) produce the same bits: ptxas may otherwise contract
 // the plain multiplies and adds into FMAs differently at each call site.  Replicated tensors rely on this -- every

@@ -214,14 +214,6 @@ __global__ void __launch_bounds__(kMapThreads) error_map_cdf_kernel(const MapGeo
   }
 }
 
-// SplitMix64: the finaliser of x + golden gamma.
-__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  uint64_t z = x + 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 __global__ void __launch_bounds__(kMapThreads) error_map_draw_kernel(const uint64_t* __restrict__ cdf, const MapGeo g,
                                                                      int64_t num_tiles, uint64_t key, int64_t num_rays,
                                                                      int64_t num_uniform, int64_t* __restrict__ out) {

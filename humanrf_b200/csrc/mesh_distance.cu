@@ -137,13 +137,6 @@ __device__ __forceinline__ float box_lower_bound(float3 p, float4 lo, float4 hi)
   return __fsub_rd(__fmul_rd(s, 0.99999904632568359375f), 1e-30f);
 }
 
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  uint64_t z = x + 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll

@@ -14,13 +14,12 @@
 //                           vertex without a mask) -> device list + device count; zeroes sigma at the other vertices
 //   density_lattice_kernel: tiles of 128 vertices, one sample each -> sigma
 //
-// The density of every sample is bit for bit what hrf_field_forward (mode 0, query form) returns for its position: the
-// same encode_to_smem, the same two wgmma layers and the same epilogue.
-#include "field_mlp.cuh"
+// The density of every sample is bit for bit what hrf_field_forward (mode 0, query form) returns for its position
+// (density_tile.cuh).
+#include "density_tile.cuh"
 
 namespace hrf {
 
-constexpr int kBakeCtasPerSm = 5;
 constexpr int64_t kBakeHeaderBytes = 256;       // device count, then the id list
 
 __global__ void __launch_bounds__(256) hull_compact_kernel(const uint8_t* __restrict__ hull, uint32_t n,
@@ -41,15 +40,6 @@ __global__ void __launch_bounds__(256) hull_compact_kernel(const uint8_t* __rest
     if (max_sigma != nullptr) max_sigma[v] = 0.f;
   }
 }
-
-// What every item shape of the tile loop reads: the field, the frame, the grid resolution and the compacted id list
-// with its device count.
-struct DensityTileArgs {
-  hrf_field f;
-  const int32_t* count;
-  const int32_t* ids;
-  int32_t frame, G;
-};
 
 // Sub-sample position along one axis: the cell-centred convention of the texture lookup the sampler emulates (voxel i
 // covers [i/G, (i+1)/G) of p + 0.5), sub-samples at 1/4 and 3/4 of the cell.
@@ -72,7 +62,7 @@ struct BakeArgs : DensityTileArgs {
     s.y = __fadd_rn(bake_coord(y, (sub >> 1) & 1, Gf), 0.5f);
     s.z = __fadd_rn(bake_coord(z, sub >> 2, Gf), 0.5f);
   }
-  __device__ __forceinline__ void store(bool valid, int32_t vid, int sub, float m, const hrf_segment* seg) const {
+  __device__ __forceinline__ void store(bool valid, int64_t, int32_t vid, int sub, float m, const hrf_segment* seg) const {
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
@@ -98,62 +88,10 @@ struct LatticeArgs : DensityTileArgs {
     s.y = __fadd_rn(__fsub_rn(__fdiv_rn((float)y, Gf), 0.5f), 0.5f);
     s.z = __fadd_rn(__fsub_rn(__fdiv_rn((float)z, Gf), 0.5f), 0.5f);
   }
-  __device__ __forceinline__ void store(bool valid, int32_t vid, int, float m, const hrf_segment*) const {
+  __device__ __forceinline__ void store(bool valid, int64_t, int32_t vid, int, float m, const hrf_segment*) const {
     if (valid) sigma[vid] = m;
   }
 };
-
-// The persistent tile loop: the item count stays on the device, every CTA walks tiles of Item::kItemsPerTile items of
-// kTile / kItemsPerTile rows each.  Only the sigma net is evaluated: its two layers are the first kWCol1 bytes of the
-// blob, whatever the colour net's width.  Fmt: the table entry format (field_common.cuh).
-template <class Item, class Fmt = TabBf16x2>
-__device__ __forceinline__ void density_tile_loop(const Item& args) {
-  extern __shared__ unsigned char smem_raw[];
-  FwdSmem& sm = *reinterpret_cast<FwdSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
-  const int tid = threadIdx.x;
-  const hrf_field& f = args.f;
-
-  if (tid == 0) {
-    mbar_init(&sm.bar_w, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&sm.bar_w, kWCol1);
-    tma_load_1d(sm.w, f.mlp_blob, kWCol1, &sm.bar_w);
-  }
-  bool weights_ready = false;
-
-  // frame -> segment and normalised local time, once (the host checked that the frame lies inside the LUT)
-  const int sg = __ldg(f.frame_to_segment + args.frame);
-  const float t_local = __ldg(f.frame_to_tlocal + args.frame);
-  const hrf_segment* seg = (sg >= 0 && sg < f.num_segments) ? f.segments + sg : nullptr;
-
-  constexpr int kRows = kTile / Item::kItemsPerTile;
-  const int64_t n = *reinterpret_cast<const volatile int32_t*>(args.count);
-  const int64_t num_tiles = (n + Item::kItemsPerTile - 1) / Item::kItemsPerTile;
-  const int slot = (int)((unsigned)tid / kRows), sub = (int)((unsigned)tid % kRows);
-  for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int64_t k = tile * Item::kItemsPerTile + slot;
-    const bool valid = k < n;
-    const int32_t id = valid ? __ldg(args.ids + k) : 0;
-    Sample s;
-    s.seg = valid ? seg : nullptr;
-    s.t = t_local;
-    args.position(id, sub, s);
-    encode_to_smem<false, 1, Fmt>(f, s, sm.a, tid);
-    if (!weights_ready) {
-      mbar_wait(&sm.bar_w, 0);
-      weights_ready = true;
-    }
-    run_hidden<false, 32>(sm, kWSig1);
-    float o[16];
-    run_layer16<false, 64>(sm, kWSig2, o);
-    // humanrf.py:184 : density = truncated_exp(h[...,0]) * density_scale, exactly the forward's epilogue
-    args.store(valid, id, sub, __expf(o[0]) * f.density_scale, seg);
-  }
-  if (!weights_ready) mbar_wait(&sm.bar_w, 0);  // never leave a bulk copy in flight
-}
 
 __global__ void __launch_bounds__(kTile, kBakeCtasPerSm) occupancy_bake_kernel(const __grid_constant__ BakeArgs args) {
   density_tile_loop(args);
@@ -170,14 +108,6 @@ __global__ void __launch_bounds__(kTile, kBakeCtasPerSm) occupancy_bake_i8_kerne
 
 __global__ void __launch_bounds__(kTile, kBakeCtasPerSm) density_lattice_i8_kernel(const __grid_constant__ LatticeArgs args) {
   density_tile_loop<LatticeArgs, TabInt8x2>(args);
-}
-
-// Dynamic shared memory of the tile loop, and its persistent grid: one full wave, capped by the tiles of a full list.
-static int density_tile_smem() { return (int)(offsetof(FwdSmem, w) + kWCol1) + 128; }
-static int density_tile_grid(int64_t max_items, int items_per_tile) {
-  const int64_t max_tiles = (max_items + items_per_tile - 1) / items_per_tile;
-  const int64_t wave = (int64_t)sm_count() * kBakeCtasPerSm;
-  return (int)(max_tiles < wave ? max_tiles : wave);
 }
 
 // out = hull AND (any live voxel in the 3x3x3 neighbourhood), one thread per voxel; `live` is 0 outside the hull.

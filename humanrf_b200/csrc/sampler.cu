@@ -22,9 +22,7 @@ namespace hrf {
 
 __global__ void pack_bits_kernel(const uint8_t* __restrict__ g, uint32_t* __restrict__ bits, int64_t n) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool v = (i < n) && (g[i] != 0);
-  const uint32_t b = __ballot_sync(0xffffffffu, v);
-  if ((threadIdx.x & 31) == 0 && i < n) bits[i >> 5] = b;
+  store_occupancy_bits(bits, i, n, (i < n) && (g[i] != 0));
 }
 
 // Emulates tex3D<float>(clamp, linear, normalised coords, normalised-float uint8) > 0.

@@ -135,6 +135,8 @@ class DataLoader:
                                                                         self.occupancy_grids_buffer_size)
         self.replacing = False
         self.ray_source = None             # TRAINING: an object whose draw(batch_size) replaces torch.randint (ErrorMap)
+        # TRAINING: an object told of every grid the ring takes, grid_added(frame, hull, handle) (TrainingOccupancy)
+        self.occupancy_source = None
         self.slot_pairs = [None] * self.buffer_size           # the (camera, frame) pair every pool slot currently holds
         self.camera_frame_pairs = self._camera_frame_pair_generator()
         for slot in range(self.buffer_size):
@@ -204,6 +206,8 @@ class DataLoader:
                 handle = self.cuda_grid_texture.add_grid(grid)
                 if self.mode == M.TRAINING:
                     self.frame_to_grid_texture[frame_number] = handle
+                    if self.occupancy_source is not None:
+                        self.occupancy_source.grid_added(frame_number, grid, handle)
             self.grid_texture_objects_cuda[buffer_index] = handle
         self.slot_pairs[buffer_index] = (int(camera_number), int(frame_number))
         self.frame_numbers_cuda[buffer_index] = frame_number

@@ -6,8 +6,9 @@ between limbs and whatever the cameras cannot rule out.  ``bake_occupancy_grid``
 such a hull and keeps only the voxels where pruning could keep a sample (include/humanrf_b200.h,
 ``hrf_bake_occupancy``), so a render evaluates far fewer candidate samples for the same image.
 
-Inference only: a training loader keeps the hull grids, because a learned grid would cull space the model has not
-learned yet.
+A grid baked once is for inference: baked from a model in training it would cull space the model has not learned yet.
+For training, ``toolbox.training_occupancy.TrainingOccupancy`` refreshes learned grids from the current field every few
+steps (DESIGN.md §3.21).
 """
 from __future__ import annotations
 
@@ -69,7 +70,8 @@ class LearnedOccupancyDataset:
     baked grid in the type and layout datasets return (numpy uint8 [G,G,G]), baked once per frame and cached.  Hand it
     to a VALIDATION or TEST ``DataLoader`` (and through it to ``Trainer.validate`` / ``Trainer.test``) to render with
     learned grids.  It is not meant for TRAINING loaders: a model in training has not learned the space yet, and a grid
-    baked from it would cull space that the hull keeps for a reason.  The cache is not refreshed when the model changes;
+    baked from it once would cull space that the hull keeps for a reason (``TrainingOccupancy`` refreshes its grids
+    while training instead).  The cache is not refreshed when the model changes;
     build a new wrapper after further training."""
 
     def __init__(self, dataset, model, render_step_size: float = 4e-4):

@@ -43,6 +43,11 @@ Error map (`error_map=`, toolbox/error_map.py ErrorMap, DESIGN.md §3.20): right
 stream, the step adds each ray's colour Huber error into its pool pixel's tile (hrf_error_map_accumulate, fed by the
 batch's pool indices `pixels`) and folds the tiles into the map (hrf_error_map_update); the loader's next draw reads it.
 Both only read the step's buffers: the field's update is the one the step makes without an error map.
+
+Training occupancy (`training_occupancy=`, toolbox/training_occupancy.py TrainingOccupancy, DESIGN.md §3.21): at the end
+of the step, after the field's Adam, its update(t) refreshes the sampler's learned occupancy grids every `interval` steps
+from its warm-up on.  It reads the updated field and writes the loader's ring slots only; with world_size > 1 every
+rank builds its own over its own loader (the replicas are bit-identical, so no collective is needed).
 """
 from __future__ import annotations
 
@@ -77,7 +82,7 @@ class FusedTrainer:
                  max_steps: int = 50001, bce_loss_weight: float = 1e-3, huber_delta: float = 0.01,
                  render_step_size: float = 4e-4, world_size: int = 1, process_group=None, prune: bool = True,
                  seed: int = 123, reuse: str = "feat", exchange: str = "p2p", overlap_exchange: bool = False,
-                 camera_poses=None, camera_responses=None, error_map=None):
+                 camera_poses=None, camera_responses=None, error_map=None, training_occupancy=None):
         """camera_poses: a toolbox.camera_refinement.CameraPoses over the loader the batches come from; its cameras'
         poses are refined with the field (then step() needs `cameras`).  Its world_size must be this trainer's: with
         world_size > 1 every rank builds its own CameraPoses over its own loader, the ranks exchange their per-camera
@@ -87,7 +92,9 @@ class FusedTrainer:
         is refined with the field (then step() needs `cameras`).  The same world_size, process_group and
         overlap_exchange rules as camera_poses.
         error_map: a toolbox.error_map.ErrorMap over the loader the batches come from (then step() needs `pixels`); with
-        world_size > 1 every rank has its own, built with its rank."""
+        world_size > 1 every rank has its own, built with its rank.
+        training_occupancy: a toolbox.training_occupancy.TrainingOccupancy over the loader the batches come from; the
+        step ends with its update(t).  With world_size > 1 every rank has its own, built with its rank."""
         from .toolbox.compact_model import require_trainable
 
         require_trainable(model, "FusedTrainer")
@@ -117,10 +124,11 @@ class FusedTrainer:
         self.overlap_exchange = bool(overlap_exchange) and self.exchange == "p2p"
         self.rank = dist.get_rank(process_group) if world_size > 1 else 0
         for name, calib in (("camera_poses", camera_poses), ("camera_responses", camera_responses),
-                            ("error_map", error_map)):
+                            ("error_map", error_map), ("training_occupancy", training_occupancy)):
             if calib is not None and calib.rank != self.rank:
                 raise ValueError(f"{name} has rank {calib.rank}, the trainer rank {self.rank}")
         self.error_map = error_map
+        self.training_occupancy = training_occupancy
         self.params: List[torch.nn.Parameter] = model.hot_parameters()
         dev = self.params[0].device
         self.dev = dev
@@ -493,6 +501,9 @@ class FusedTrainer:
             if resp is not None and self.world == 1:
                 launches += resp.step(t_done)
                 mark("response_step")
+        if self.training_occupancy is not None:
+            launches += self.training_occupancy.update(self.t)
+            mark("training_occupancy")
         self.last = {"samples": count[0] if count is not None else n_cap, "loss": loss[0], "marks": marks}
         if return_loss:
             return float(loss.item())

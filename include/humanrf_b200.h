@@ -925,6 +925,45 @@ int hrf_error_map_reset_slots(const hrf_error_map_geometry* geometry, int64_t fi
                               float prior, float* ema /* [tiles] */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Occupancy grids of the training sampler learned while training (toolbox/training_occupancy.py TrainingOccupancy,
+ * DESIGN.md §3.21).  Per frame f, from its hull (uint8 [G][G][G] indexed [z][y][x], non-zero = occupied):
+ *   1. ids: the hull's voxel indices z G^2 + y G + x, int32, ascending (hrf_training_occupancy_compact).  The caller
+ *      reads the device count back once per newly seen frame to size ids and bound.
+ *   2. bound: float32 per listed voxel, starting at +inf (a voxel never evaluated is live).
+ *   3. evaluate (refresh counter c, seed s; hrf_training_occupancy_update):
+ *        key = S(S(S(s) ^ f) ^ c) (hrf_training_occupancy_key), S the SplitMix64 finaliser of x + 0x9E3779B97F4A7C15,
+ *        h = S(key ^ id), g = S(h); u_x = (h >> 40) 2^-24, u_y = ((h >> 16) & (2^24 - 1)) 2^-24, u_z = (g >> 40) 2^-24;
+ *        px = __fsub_rn(__fdiv_rn(__fadd_rn((float)x, u_x), (float)G), 0.5f), the same for y and z (the bake's
+ *        cell-centred convention with a hashed offset; the rounding of x + u_x can put the point on the voxel's upper
+ *        face);
+ *        sigma = exactly what hrf_field_forward (mode 0, query form) returns at p and frame f;
+ *        bound = !isfinite(sigma) ? +inf : isinf(bound) ? sigma : fmaxf(__fmul_rn(decay, bound), sigma).
+ *   4. pack (hrf_training_occupancy_pack): live <=> 1.f - expf(-bound * step) >= alpha_thre (the bake's alpha test);
+ *      grid = hull AND dilate(live), a 26-neighbourhood dilation by one voxel that never leaves the hull, the hull
+ *      rebuilt from ids; written in place into an occupancy ring slot (the handle of hrf_occgrid_add, ceil(G^3 / 32)
+ *      words) in hrf_occgrid_add's bit layout: voxel i is bit i & 31 of word i >> 5.  The ring does not advance.
+ * G in [1, 1024].  Every entry is asynchronous on `stream` and reads nothing back.  workspace:
+ * hrf_training_occupancy_workspace_bytes(G) bytes of device scratch, shared by compact and pack.
+ * ---------------------------------------------------------------------------------------- */
+uint64_t hrf_training_occupancy_key(uint64_t seed, int32_t frame_number, uint64_t counter);
+int64_t hrf_training_occupancy_workspace_bytes(int grid_resolution);
+/* Writes *count (device int32) and, when ids is not NULL, the ids (capacity: the count). */
+int hrf_training_occupancy_compact(const uint8_t* hull_u8 /* [G^3] */, int grid_resolution, int32_t* ids /* or NULL */,
+                                   int32_t* count /* [1] device */, void* workspace, void* stream);
+/* One launch over the num_ids listed voxels (num_ids: the count compact wrote, which `count` holds on the device).
+ * points (optional, float32 [num_ids, 3]) receives p.  Needs a bf16-table field and the frame inside its frame table;
+ * decay in (0, 1]. */
+int hrf_training_occupancy_update(const hrf_field* f, int32_t frame_number, int grid_resolution,
+                                  const int32_t* ids /* [num_ids] */, const int32_t* count /* [1] device */,
+                                  int64_t num_ids, uint64_t seed, uint64_t counter, float decay,
+                                  float* bound /* [num_ids] */, float* points /* [num_ids, 3] or NULL */, void* stream);
+/* counts (optional, int64 [2] device): {live voxels, set bits of the grid}. */
+int hrf_training_occupancy_pack(const int32_t* ids /* [num_ids] */, const float* bound /* [num_ids] */,
+                                int64_t num_ids, int grid_resolution, float step, float alpha_thre,
+                                uint32_t* slot_bits /* [ceil(G^3 / 32)] */, int64_t* counts /* [2] or NULL */,
+                                void* workspace, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Self tests (used by tests/ only): one 128xN x K (or 64xNxK) wgmma with caller-chosen descriptor
  * fields, to pin the shared-memory descriptor encoding on real hardware.
  * ---------------------------------------------------------------------------------------- */
